@@ -114,19 +114,21 @@ __global__ void gen_kernel(long long n_part, long long n_supp, long long n_cust,
 }
 }  // namespace
 
+static const long long kMaxGrid = 132 * 16;      // grid-stride launches: 16 CTAs on each of an H100's 132 SMs
+
 extern "C" {
 
 // lines[r] = number of lineitems of order row first + r (device array of n ints)
 int tpch_gpu_count_lines(long long first, long long n, int* lines, void* stream) {
   if (n <= 0) return 0;
-  const int grid = (int)((n + 255) / 256 < 148 * 16 ? (n + 255) / 256 : 148 * 16);
+  const int grid = (int)((n + 255) / 256 < kMaxGrid ? (n + 255) / 256 : kMaxGrid);
   count_lines_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(first, n, lines);
   return (int)cudaGetLastError();
 }
 // offs[r] = exclusive prefix of lines[] (device array of n int64); counts as in tpch_counts_get()
 int tpch_gpu_generate(long long n_part, long long n_supp, long long n_cust, long long first, long long n, const long long* offs, const TpchGpuOut* out, void* stream) {
   if (n <= 0) return 0;
-  const int grid = (int)((n + 127) / 128 < 148 * 16 ? (n + 127) / 128 : 148 * 16);
+  const int grid = (int)((n + 127) / 128 < kMaxGrid ? (n + 127) / 128 : kMaxGrid);
   gen_kernel<<<grid, 128, 0, (cudaStream_t)stream>>>(n_part, n_supp, n_cust, first, n, offs, *out);
   return (int)cudaGetLastError();
 }

@@ -27,12 +27,20 @@ class _Out(ctypes.Structure):
     _fields_ = [(f, ctypes.c_void_p) for f in _FIELDS]
 
 
+_ARCH = "arch=compute_90a,code=sm_90a"
+
+
 def build(force: bool = False) -> str:
     src = os.path.join(_HERE, "tpch_dbgen_gpu.cu")
+    stamp = _SO + ".arch"
+    if not os.path.exists(stamp) or open(stamp).read() != _ARCH:
+        force = True        # a library built for another architecture
     if force or not os.path.exists(_SO) or os.path.getmtime(_SO) < os.path.getmtime(src):
         os.makedirs(os.path.dirname(_SO), exist_ok=True)
         nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-        subprocess.check_call([nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-shared", "-o", _SO, src, "-lcudart"])
+        subprocess.check_call([nvcc, "-gencode", _ARCH, "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-shared", "-o", _SO, src, "-lcudart"])
+        with open(stamp, "w") as f:
+            f.write(_ARCH)
     return _SO
 
 

@@ -1,5 +1,5 @@
 /*
- * sailgpu.h -- C ABI of libsailgpu.so: the B200-native replacement for the DataFusion physical
+ * sailgpu.h -- C ABI of libsailgpu.so: the H100-native replacement for the DataFusion physical
  * operators on Sail's hot path.
  *
  * Who binds this.  A Rust shim crate inside Sail (see INTEGRATION.md) implements
@@ -208,7 +208,7 @@ SAILGPU_API int32_t sailgpu_parquet_inspect(const struct ArrowSchema* schema, co
                                             int64_t n_rows, int32_t column, char* buf, size_t cap);
 
 /* Plan-time kernel specialisation.  The library interprets any pipeline at once and, for pipelines that see enough
- * rows (SAILGPU_JIT_MIN_ROWS, default 4 Mi), compiles a specialised sm_100a kernel with NVRTC the first time; the
+ * rows (SAILGPU_JIT_MIN_ROWS, default 4 Mi), compiles a specialised sm_90a kernel with NVRTC the first time; the
  * cubin is cached next to the library (or in $SAILGPU_JIT_CACHE).  This call moves that compilation to planning time
  * (the rewrite pass knows the pipelines of a query before the first batch): it generates the kernel for `spec` as it
  * would run over batches whose column i carries a validity buffer iff bit i of `validity_mask` is set, and with
@@ -282,8 +282,8 @@ SAILGPU_API void sailgpu_host_free(sailgpu_ctx* ctx, void* p);
 /* Environment (read by the library; all optional, none changes results):
  *   SAILGPU_JIT=0                 interpret every pipeline;  SAILGPU_JIT_MIN_ROWS=n  rows a pipeline must have seen before it is specialised
  *   SAILGPU_JIT_CACHE=dir         where cubins are kept;  SAILGPU_JIT_VERBOSE / _STRICT / _DUMP  diagnostics of the specialiser
- *   SAILGPU_JIT_PROBE=1           specialise hash-join probe pipelines too (measured slower than the interpreter: off)
- *   SAILGPU_DIRECT_KEY=1          direct-key protocol for single-word group keys (measured slower end to end: off)
+ *   SAILGPU_JIT_PROBE=1           specialise hash-join probe pipelines too (slower than the interpreter as tuned: off)
+ *   SAILGPU_DIRECT_KEY=1          direct-key protocol for single-word group keys (slower end to end as tuned: off)
  *   SAILGPU_NO_JOIN_SWAP=1        never exchange the roles of a join's inputs;  SAILGPU_TOPK_MIN_ROWS=n  TopK selection threshold
  *   SAILGPU_PACK_THREADS=n        packer threads of the host ingest (default: the CPUs the cgroup grants, at most 32)
  *   SAILGPU_H2D_PACK=0 / SAILGPU_PACK_ONE_PASS=0 / SAILGPU_PACK_PIECE_ROWS=n / SAILGPU_PACK_NUMA=0 / SAILGPU_PACK_DRY=1   ingest A/B knobs

@@ -72,7 +72,7 @@ SAILGPU_API int32_t sailgpu_ctx_create(int32_t device, sailgpu_ctx** out) {
     SG_CUDA(cudaSetDevice(device));
     cudaDeviceProp prop;
     SG_CUDA(cudaGetDeviceProperties(&prop, device));
-    SG_CHECK(prop.major >= 10, SAILGPU_ERR_NO_DEVICE, std::string("device '") + prop.name + "' is not sm_100-class; this library only carries sm_100a code");
+    SG_CHECK(prop.major == 9 && prop.minor == 0, SAILGPU_ERR_NO_DEVICE, std::string("device '") + prop.name + "' is not sm_90 (Hopper); this library only carries sm_90a code");
     c->ctx.sm_count = prop.multiProcessorCount;
     c->ctx.max_smem = prop.sharedMemPerBlockOptin;
     SG_CUDA(cudaStreamCreateWithFlags(&c->ctx.stream, cudaStreamNonBlocking));

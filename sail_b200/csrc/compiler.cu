@@ -463,14 +463,14 @@ void PipelineCompiler::finalize(CompiledPipeline& out, Ctx* ctx, int hot_wanted)
     return fixed + *temps + ((out.extra_scratch + 127) & ~127u) + (size_t)stages * s;
   };
   const int force_rpt = env_int("SAILGPU_RPT", 0), force_stages = env_int("SAILGPU_STAGES", 0), force_hot = env_int("SAILGPU_HOT", -1);
-  // (rows per thread, input stages) in measured order of preference on B200 (scripts/sweep_q1.py, scripts/bench_ops.py):
+  // (rows per thread, input stages) in order of preference, as swept with scripts/sweep_q1.py and scripts/bench_ops.py (the
+  // order was tuned before the move to H100 and has not been swept there again):
   // aggregation wants 2 CTAs/SM of 512-row tiles; plain projection streams best with big double-buffered tiles;
   // compaction / join / partition sinks prefer big single-stage tiles and more resident CTAs
   static const int C_AGG[][2] = {{2, 1}, {1, 2}, {2, 2}, {1, 1}, {4, 1}, {4, 2}};
   // with the kernel specialiser on, dictionary aggregation uses 256-row tiles: the specialised kernel (which inherits the tile
-  // size so that tile lists stay valid across both kernels) keeps one row per thread in registers without spills -- measured on
-  // Q1 SF10: 1.49 ms against 1.95 ms with two rows per thread (profiles/r02_jit_sweep.txt); the interpreter, which now only sees
-  // small inputs, loses a few percent
+  // size so that tile lists stay valid across both kernels) keeps one row per thread in registers without spills, which
+  // beat two rows per thread on Q1; the interpreter, which now only sees small inputs, loses a few percent
   static const int C_AGG_JIT[][2] = {{1, 2}, {1, 1}, {2, 1}, {2, 2}, {4, 1}, {4, 2}};
   // high-cardinality aggregation is bound by the latency of the global table: small tiles, 4 CTAs/SM (64 registers)
   static const int C_AGG_COLD[][2] = {{2, 1}, {2, 2}, {1, 2}, {1, 1}, {4, 1}, {4, 2}};

@@ -1,4 +1,4 @@
-// dev_util.cuh -- sm_100a device helpers: mbarrier + TMA bulk copy, 128-bit integers, hashing.
+// dev_util.cuh -- sm_90a device helpers: mbarrier + TMA bulk copy, 128-bit integers, hashing.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

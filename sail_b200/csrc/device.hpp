@@ -27,7 +27,7 @@ struct PackPool;
 
 struct Ctx {
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   size_t max_smem = 227 * 1024;
   cudaStream_t stream = nullptr;        // compute stream
   // compiled pipelines shared by every operator instance created from the same spec over the same schema (engine.cu): an
@@ -57,7 +57,7 @@ struct Ctx {
   // so a block released by the host can be handed to the next request of its size class at once: its new first use is
   // ordered after the old last use.  Operators re-allocate the same sizes batch after batch; going to the driver's
   // pool each time costs microseconds per call and, when differently sized operators alternate, fresh mappings of
-  // gigabytes (measured: a 6 ms join took 20 ms after an aggregation had reshaped the pool).
+  // gigabytes (a join became several times slower after an aggregation had reshaped the pool).
   std::mutex cache_mu;
   std::unordered_map<size_t, std::vector<void*>> cache;
   size_t cached_bytes = 0;

@@ -186,7 +186,7 @@ struct PipelineOp : Op {
   // ---- two-pass filter ---------------------------------------------------------------------------
   // An order-preserving single-pass compaction chains every tile to all earlier ones (decoupled look-back), and since a
   // tile only knows its count after evaluating the predicate the chain runs at the pace of the slowest resident tile
-  // (profiles/: ~45 % of the FilterExec kernel's stall samples).  Large batches therefore take two passes: pass 1
+  // (the largest share of the FilterExec kernel's stall samples).  Large batches therefore take two passes: pass 1
   // reads only the predicate's columns and stores the mask (1 bit / row); the per-tile popcounts are scanned; pass 2
   // reads the projected columns + mask and stores every tile at its known offset, tiles in any order.
   static constexpr int64_t TWO_PASS_MIN_ROWS = 1 << 18;
@@ -274,11 +274,11 @@ struct PipelineOp : Op {
     A.n_groups = run.scal.n_groups();
     A.direct_key = tab.direct ? 1 : 0;
   }
-  // One never-null 8-byte key word: the table CAN take the direct-key protocol.  Opt-in (SAILGPU_DIRECT_KEY=1): measured on
-  // GROUP BY l_orderkey over SF10 (60 M rows -> 15 M groups) the insert kernel itself did not get faster without the fence and the
-  // counter round trip (6.25 vs 6.5 ms: it is bound by the per-row accumulator atomics that need their old value for the 128-bit
-  // carry), while initialising and scanning every ENTRY of the 64 M-slot table cost 4.3 ms more than the 4-byte state words of
-  // the general protocol (11.5 vs 8.4 ms per aggregation, profiles/README.md).
+  // One never-null 8-byte key word: the table CAN take the direct-key protocol.  Opt-in (SAILGPU_DIRECT_KEY=1): on GROUP BY
+  // l_orderkey over SF10 (60 M rows -> 15 M groups) the insert kernel itself did not get faster without the fence and the counter
+  // round trip (it is bound by the per-row accumulator atomics that need their old value for the 128-bit carry), while
+  // initialising and scanning every ENTRY of the 64 M-slot table costs more than the 4-byte state words of the general protocol
+  // (as tuned; not re-measured on H100).
   static bool direct_eligible(const AggParams& A) {
     const char* e = getenv("SAILGPU_DIRECT_KEY");
     return A.n_keys == 1 && A.key_words == 1 && !A.has_null_word && e && *e && atoi(e) != 0;
@@ -556,9 +556,9 @@ struct PipelineOp : Op {
 
 // Plan-time specialisation (sailgpu_jit_precompile): compiles the pipeline of `spec` for a batch whose columns carry
 // validity buffers where `validity_mask` has a bit set, writes the specialised kernel's source to *source and, with
-// `compile`, its cubin into the kernel cache -- all without a device (NVRTC cross-compiles for sm_100a).
+// `compile`, its cubin into the kernel cache -- all without a device (NVRTC cross-compiles for sm_90a).
 size_t pipeline_precompile(const Json& spec, const std::vector<Schema>& inputs, uint64_t validity_mask, bool cold, bool compile, std::string* source) {
-  static Ctx plan_ctx;      // B200 geometry (148 SMs, 227 KB of shared memory per CTA); never touches a device
+  static Ctx plan_ctx;      // H100 geometry (132 SMs, 227 KB of shared memory per CTA); never touches a device
   std::unique_ptr<Op> op = make_op(&plan_ctx, spec, inputs, 0);
   PipelineOp* p = dynamic_cast<PipelineOp*>(op.get());
   SG_CHECK(p != nullptr, SAILGPU_ERR_UNSUPPORTED, "only filter / projection / aggregate pipelines are specialised");
@@ -579,7 +579,7 @@ size_t pipeline_precompile(const Json& spec, const std::vector<Schema>& inputs, 
 }
 
 // Plan-time limits of a filter / projection / aggregate pipeline (sailgpu_spec_validate): the tile program is compiled against the
-// B200 geometry for a batch without validity buffers, so that the data-independent limits -- "more than 6 group keys", "group key
+// H100 geometry for a batch without validity buffers, so that the data-independent limits -- "more than 6 group keys", "group key
 // wider than 64 bytes", "does not fit in shared memory" ... -- are answered while planning, never after the first batch arrived.
 // (Validity buffers add one column buffer each; a batch whose nullable columns push a pipeline over the 20-buffer limit is still
 // reported at push time as SAILGPU_ERR_UNSUPPORTED.)  Touches no device.

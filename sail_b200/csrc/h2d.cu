@@ -4,6 +4,7 @@
 // crosses per RecordBatch (SURVEY.md section 8b): Arrow's fixed widths are an in-memory format, not a wire format.
 #include <climits>
 #include "h2d.hpp"
+#include "kernels.hpp"
 
 #include <sched.h>
 #include <sys/syscall.h>
@@ -20,8 +21,8 @@ namespace {
 constexpr int64_t MAX_PIECE_ROWS = 256 * 1024;
 constexpr size_t SLOT_BYTES = (size_t)MAX_PIECE_ROWS * 16;     // 4 MiB: one piece of the widest column
 // rows per piece: SAILGPU_PACK_PIECE_ROWS (a multiple of 1024, at most 256 Ki).  Every piece costs three driver calls (copy, expand
-// kernel, event) that serialise across the packer threads: 64 Ki-row pieces spent a third of the import there (55 vs 42 ms for a
-// 60 M-row batch, profiles/r02_h2d_probe.txt); the one-pass packer no longer needs the piece to stay in L2 for a second loop
+// kernel, event) that serialise across the packer threads, so small pieces spend a large share of the import there;
+// the one-pass packer no longer needs the piece to stay in L2 for a second loop
 static int64_t piece_rows() {      // read per batch: A/B measurements in one process
   const char* e = getenv("SAILGPU_PACK_PIECE_ROWS");
   const int64_t r = e && *e ? atoll(e) : MAX_PIECE_ROWS;
@@ -200,10 +201,9 @@ struct PackPool {
   bool stop = false;
   std::string error;
   // NUMA (SAILGPU_PACK_NUMA=0 turns it off): the packers run on the CPUs of the node the producer's pages live on.  A reader on
-  // the other socket gets ~60 % of the local bandwidth (52 vs 32 ms for the host side of a 60 M-row batch).  In a small probe
-  // process the scheduler happens to keep the threads near the data and binding is neutral (37.7 vs 36.7 ms), but in bench.py --
-  // host tables first touched by the main thread, packers created later -- it is 75.8 vs 103.7 ms per two-batch step
-  // (profiles/README.md).
+  // the other socket gets only part of the local bandwidth.  In a small probe process the scheduler happens to keep the
+  // threads near the data and binding is neutral, but in bench.py -- host tables first touched by the main thread, packers
+  // created later -- binding is what keeps the packers next to their data.
   cpu_set_t allowed;                         // the process's affinity when the pool was created
   std::vector<cpu_set_t> node_cpus;          // allowed CPUs of every NUMA node (empty sets: unknown)
   std::atomic<int> want_node{-1};
@@ -253,7 +253,7 @@ struct PackPool {
     } else {
       e = cudaMemcpyAsync(s.dev, s.host, pk.bytes, cudaMemcpyHostToDevice, w.stream);
       if (e == cudaSuccess) {
-        const int grid = (int)std::min<int64_t>((it.n + 255) / 256, 148 * 4);
+        const int grid = (int)std::min<int64_t>((it.n + 255) / 256, grid_cap(4));
         if (pk.enc == ENC_INT) unpack_int_kernel<<<grid, 256, 0, w.stream>>>(s.dev, it.dst, it.n, pk.w, it.width, pk.base);
         else unpack_view_kernel<<<grid, 256, 0, w.stream>>>(s.dev, reinterpret_cast<ulonglong2*>(it.dst), it.n, pk.w);
         e = cudaGetLastError();

@@ -145,7 +145,7 @@ static void packchk_dec128_avx512(uint8_t* __restrict out, const int64_t* __rest
   __m512i vmn = _mm512_set1_epi64(INT64_MAX), vmx = _mm512_set1_epi64(INT64_MIN), vbad = _mm512_setzero_si512();
   int64_t i = 0;
   for (; i + 16 <= n; i += 16) {
-    // a core's line-fill buffers alone sustain ~10 GB/s from DRAM; software prefetches 4 KB ahead add another 20 % (measured)
+    // a core's line-fill buffers alone limit what one thread streams from DRAM; software prefetches 4 KB ahead add to it
     { const char* pf = reinterpret_cast<const char*>(p + 2 * i) + 4096;
       _mm_prefetch(pf, _MM_HINT_T0); _mm_prefetch(pf + 64, _MM_HINT_T0); _mm_prefetch(pf + 128, _MM_HINT_T0); _mm_prefetch(pf + 192, _MM_HINT_T0); }
     const __m512i a0 = _mm512_loadu_si512(p + 2 * i), a1 = _mm512_loadu_si512(p + 2 * i + 8), a2 = _mm512_loadu_si512(p + 2 * i + 16), a3 = _mm512_loadu_si512(p + 2 * i + 24);

@@ -1,10 +1,10 @@
 // jit.cu -- pipeline specialiser (host side).
 //
 // The interpreter (pipeline.cu) runs any fused Filter -> Projection -> Aggregate chain at once; its cost is ~650 thread
-// instructions per TPC-H Q1 row, most of them descriptor decoding and shared-memory round trips of intermediates
-// (profiles/README.md).  For pipelines that see enough rows this file writes the same pipeline as straight-line CUDA
+// instructions per TPC-H Q1 row, most of them descriptor decoding and shared-memory round trips of intermediates.
+// For pipelines that see enough rows this file writes the same pipeline as straight-line CUDA
 // over registers -- one `struct G` per pipeline, consumed by the templates in jit_rt.cuh -- and compiles it with NVRTC
-// for sm_100a.  No new operator semantics live here: every generated statement is the register form of one VM
+// for sm_90a.  No new operator semantics live here: every generated statement is the register form of one VM
 // instruction (vm.h) or one sink descriptor.  Kernels are cached by source hash, in memory and as cubins next to the
 // library (sail_b200/_build/jit_cache), so a pipeline is compiled once per machine.
 #include "jit.hpp"
@@ -414,8 +414,8 @@ bool jit_supported(const CompiledPipeline& cp, std::string* why) {
   if (cp.sink != SINK_AGG && cp.sink != SINK_STORE && cp.sink != SINK_COMPACT) return no("sink is not aggregate / store / compact");
   if (cp.jit.inputs.empty()) return no("pipeline reads no column");
   if (cp.n_probes > 0) {      // hash-join probe pipelines: one key of at most 8 bytes per probe (the PK-FK joins); store / compact sinks
-    // Opt-in (SAILGPU_JIT_PROBE=1): correct (the relational suite passes with it), but measured SLOWER than the interpreter on
-    // orders x lineitem at SF10 (6.5 vs 5.5 ms): the interpreter's probe issues the first-slot loads of all rows of a thread
+    // Opt-in (SAILGPU_JIT_PROBE=1): correct (the relational suite passes with it), but slower than the interpreter on
+    // orders x lineitem when it was tuned (not re-measured on H100): the interpreter's probe issues the first-slot loads of all rows of a thread
     // before the dependent key loads, the generated code resolves one row at a time -- latency, not instructions, bounds a probe.
     static const bool on = getenv("SAILGPU_JIT_PROBE") != nullptr && atoi(getenv("SAILGPU_JIT_PROBE")) != 0;
     if (!on) return no("join probes run on the interpreter (SAILGPU_JIT_PROBE=1 specialises them)");
@@ -547,9 +547,10 @@ uint64_t fnv1a(const std::string& s, uint64_t seed) {
   for (unsigned char c : s) { h ^= c; h *= 0x100000001b3ull; }
   return h;
 }
-std::string runtime_fingerprint() {       // the embedded headers are part of every kernel's identity
+static const char kJitArch[] = "sm_90a";
+std::string runtime_fingerprint() {       // the target architecture and the embedded headers are part of every kernel's identity
   static const std::string fp = [] {
-    std::string all;
+    std::string all = kJitArch;
     for (const EmbeddedHeader* h = kJitHeaders; h->name; ++h) { all += h->name; all += h->text; }
     char b[40]; snprintf(b, sizeof b, "%016llx", (unsigned long long)fnv1a(all, 17));
     return std::string(b);
@@ -587,7 +588,8 @@ std::string jit_compile_cubin(const std::string& source) {
   void* prog = nullptr;
   int rc = n.CreateProgram(&prog, source.c_str(), "sg_jit_kernel.cu", (int)names.size(), texts.data(), names.data());
   SG_CHECK(rc == 0, SAILGPU_ERR_CUDA, std::string("nvrtcCreateProgram: ") + n.GetErrorString(rc));
-  const char* opts[] = {"--gpu-architecture=sm_100a", "--std=c++17", "-lineinfo", "-default-device", "--device-int128"};
+  const std::string arch = std::string("--gpu-architecture=") + kJitArch;
+  const char* opts[] = {arch.c_str(), "--std=c++17", "-lineinfo", "-default-device", "--device-int128"};
   rc = n.CompileProgram(prog, 5, opts);
   if (rc != 0) {
     size_t ls = 0; n.GetProgramLogSize(prog, &ls);

@@ -1,4 +1,4 @@
-// jit.hpp -- pipeline specialiser: CompiledPipeline -> CUDA source -> NVRTC (sm_100a) -> loaded kernel.
+// jit.hpp -- pipeline specialiser: CompiledPipeline -> CUDA source -> NVRTC (sm_90a) -> loaded kernel.
 #pragma once
 #include <string>
 
@@ -29,7 +29,7 @@ bool jit_supported(const CompiledPipeline& cp, std::string* why);
 bool jit_plan(const CompiledPipeline& cp, size_t max_smem, JitPlan* plan);
 // CUDA source of the specialised kernel (host only: needs no device)
 std::string jit_generate(const CompiledPipeline& cp, const JitPlan& plan);
-// NVRTC-compiles `source` for sm_100a; returns the cubin bytes or throws sg::Error with the compiler log
+// NVRTC-compiles `source` for sm_90a; returns the cubin bytes or throws sg::Error with the compiler log
 std::string jit_compile_cubin(const std::string& source);
 // cached (memory, then <lib dir>/jit_cache) compile + load; needs a current CUDA context
 std::shared_ptr<JitKernel> jit_get_kernel(const CompiledPipeline& cp, size_t max_smem);

@@ -2,7 +2,7 @@
 //
 // pipeline.cu interprets a fused Filter -> Projection -> Aggregate chain (a tile VM over shared-memory slots, sinks
 // driven by descriptors).  For inputs that are worth a second of compilation the host generates, per distinct pipeline,
-// a struct `G` (jit.cu) and compiles `jit_main<G>` with NVRTC for sm_100a: expressions become straight-line register
+// a struct `G` (jit.cu) and compiles `jit_main<G>` with NVRTC for sm_90a: expressions become straight-line register
 // code (no slots, no dispatch), every descriptor a compile-time constant, and the tile loop becomes an mbarrier ring of
 // TMA stages without a CTA-wide barrier per tile (warps drift independently; thread 0 re-arms a stage as soon as all
 // eight warps have released it).  The kernel argument block (KernelArgs) is the interpreter's: the generated code reads
@@ -393,7 +393,7 @@ __device__ __forceinline__ void jit_cold_rows(const KernelArgs& K, const typenam
       uint64_t* e = jit_find_or_insert_warp<G>(A, kw, hh[k], cold, K.P[0].error_flag);
       // Rows of one group that sit in the same warp (clustered inputs: the 1-7 lineitems of an order are neighbours) are combined
       // in registers first: one set of accumulator atomics per (warp, group) instead of per row.  The atomics are what bounds this
-      // path -- every accumulator adds ~1.5 ms per 60 M rows on top of the 3.5 ms of the inserts (profiles/README.md).
+      // path -- every accumulator adds atomics on top of the inserts.
       const bool upd = cold && e != nullptr;
       const unsigned lane = threadIdx.x & 31;
       const unsigned peers = __match_any_sync(0xFFFFFFFFu, upd ? reinterpret_cast<unsigned long long>(e) : (0xFFFFFFFF00000000ull | lane));

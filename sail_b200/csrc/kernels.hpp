@@ -6,6 +6,16 @@
 
 namespace sg {
 
+// Grid of a grid-stride launch: at most `per_sm` CTAs on every SM of the current device.
+inline int grid_cap(int per_sm) {
+  static const int sms = [] {
+    int d = 0, n = 0;
+    if (cudaGetDevice(&d) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, d) != cudaSuccess || n <= 0) n = 132;
+    return n;
+  }();
+  return sms * per_sm;
+}
+
 struct AggOutCol {
   int32_t kind;        // 0 group key i, 1 accumulator state/final j, 2 avg(sum acc j, count acc k)
   int32_t a, b;

@@ -245,7 +245,7 @@ struct JoinOp : Op {
   // ---- duplicate-heavy build side met by a tiny probe batch: execute with the roles exchanged --------------------------
   // The duplicate path walks, for every probe row, the chain of build rows with its key -- one thread per probe row.  With
   // a handful of probe rows against millions of build rows (the plans put the growing intermediate on the build side:
-  // TPC-H Q5 / Q7 join it with `nation`) that is a serial walk of ~10^6 dependent loads (measured 560 ms).  An inner join
+  // TPC-H Q5 / Q7 join it with `nation`) that is a serial walk of ~10^6 dependent loads.  An inner join
   // is symmetric, so such a batch runs through a nested join that builds on the probe batch and streams the build side:
   // key pairs, residual filter and projection are re-indexed, the output schema is unchanged.  Output order follows the
   // streamed side (INTEGRATION.md: the join reports maintains_input_order = false).
@@ -1810,7 +1810,7 @@ BatchPtr exchange_batches(Ctx* ctx, const Schema& schema, const std::vector<Batc
   }
   // Small messages can travel PACKED: all column buffers of one (source, destination) pair in one staging buffer, one
   // ncclSend/ncclRecv per pair instead of 2-3 per column.  Both sides derive the same layout from the all-gathered table.
-  // Opt-in (SAILGPU_PACKED_EXCHANGE=1): measured at N=4 it did not pay (4.70 vs 4.45 ms/step).
+  // Opt-in (SAILGPU_PACKED_EXCHANGE=1): at N=4 it did not pay when it was tuned (not re-measured on H100).
   constexpr int64_t PACK_LIMIT = 1 << 20;
   auto a16 = [](int64_t v) { return (v + 15) & ~(int64_t)15; };
   auto msg_bytes = [&](int src, int dst) {

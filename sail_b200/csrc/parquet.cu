@@ -398,7 +398,7 @@ DevColumn decode_parquet_column(Ctx* ctx, const Field& f, const ParquetColumnDes
     std::vector<int64_t> starts(runs.size());
     for (size_t i = 0; i < runs.size(); ++i) starts[i] = runs[i].out_start;
     BufPtr druns = upload_vec(ctx, runs.data(), runs.size() * sizeof(Run)), dstarts = upload_vec(ctx, starts.data(), starts.size() * 8);
-    expand_runs_kernel<<<(int)std::min<int64_t>((n + 255) / 256, 148 * 8), 256, 0, ctx->stream>>>(dbase, static_cast<const Run*>(druns->ptr), static_cast<const int64_t*>(dstarts->ptr),
+    expand_runs_kernel<<<(int)std::min<int64_t>((n + 255) / 256, grid_cap(8)), 256, 0, ctx->stream>>>(dbase, static_cast<const Run*>(druns->ptr), static_cast<const int64_t*>(dstarts->ptr),
                                                                                                 (int)runs.size(), n, static_cast<uint32_t*>(out->ptr));
     SG_CUDA(cudaGetLastError());
     SG_CUDA(cudaStreamSynchronize(ctx->stream));      // `starts` / `runs` are host vectors
@@ -436,7 +436,7 @@ DevColumn decode_parquet_column(Ctx* ctx, const Field& f, const ParquetColumnDes
     qsegs = upload_vec(ctx, ds.data(), sizeof(Segment));
     Q.segs = static_cast<const Segment*>(qsegs->ptr); Q.n_segs = 1;
     ddict = dev_alloc(ctx, (size_t)std::max<int64_t>(dict_count, 1) * out_width);
-    if (dict_count) decode_values_kernel<<<(int)std::min<int64_t>((dict_count + 255) / 256, 148 * 4), 256, 0, ctx->stream>>>(Q, static_cast<uint8_t*>(ddict->ptr));
+    if (dict_count) decode_values_kernel<<<(int)std::min<int64_t>((dict_count + 255) / 256, grid_cap(4)), 256, 0, ctx->stream>>>(Q, static_cast<uint8_t*>(ddict->ptr));
     SG_CUDA(cudaGetLastError());
     SG_CUDA(cudaStreamSynchronize(ctx->stream));
     didx = expand(index_runs, dense_done);
@@ -451,7 +451,7 @@ DevColumn decode_parquet_column(Ctx* ctx, const Field& f, const ParquetColumnDes
   dsegs = upload_vec(ctx, segs.data(), segs.size() * sizeof(Segment));
   D.segs = static_cast<const Segment*>(dsegs->ptr); D.n_segs = (int)segs.size();
   col.data = dev_alloc(ctx, (size_t)n_rows * out_width);
-  if (n_rows) decode_values_kernel<<<(int)std::min<int64_t>((n_rows + 255) / 256, 148 * 8), 256, 0, ctx->stream>>>(D, static_cast<uint8_t*>(col.data->ptr));
+  if (n_rows) decode_values_kernel<<<(int)std::min<int64_t>((n_rows + 255) / 256, grid_cap(8)), 256, 0, ctx->stream>>>(D, static_cast<uint8_t*>(col.data->ptr));
   SG_CUDA(cudaGetLastError());
   if (is_str) col.heaps = {dchunk};                 // long views point into the chunk bytes
   col.null_count = 0;

@@ -1533,7 +1533,7 @@ __device__ __forceinline__ uint8_t* build_find_or_claim(const BuildParams& B, co
 // CTA chain cache (shared memory, lives for the whole kernel): chains for keys that already own a slot are collected
 // per CTA and pushed on the slot once -- at the end of the kernel, or when the cache runs full.  A build side with a
 // handful of distinct keys (a fact-like intermediate joined to a dimension: TPC-H Q5 / Q7 shapes) otherwise funnels
-// millions of atomic exchanges into a few addresses (measured 37 ns each: 560 ms for an 18 M-row build).
+// millions of atomic exchanges into a few addresses.
 struct ChainCacheEntry { unsigned long long slot, first; long long last; };
 constexpr int CHAIN_CACHE_ENTRIES = 512;
 __device__ __forceinline__ bool chain_cache_push(const BuildParams& B, ChainCacheEntry* cache, uint32_t* count, uint8_t* slot, long long first, long long last) {
@@ -2142,37 +2142,37 @@ __global__ void tile_popcount_kernel(const uint32_t* __restrict__ bits, int64_t 
 }
 cudaError_t launch_tile_popcount(const uint32_t* bits, int64_t n_rows, int tile_rows, int64_t n_tiles, uint32_t* counts, cudaStream_t s) {
   if (n_tiles == 0) return cudaSuccess;
-  const int grid = (int)std::min<int64_t>((n_tiles * 32 + 255) / 256, 148 * 8);
+  const int grid = (int)std::min<int64_t>((n_tiles * 32 + 255) / 256, grid_cap(8));
   tile_popcount_kernel<<<grid, 256, 0, s>>>(bits, n_rows, tile_rows, n_tiles, counts);
   return cudaGetLastError();
 }
 
 cudaError_t launch_agg_rehash(const AggParams& A, const uint8_t* old_table, const uint32_t* old_occ, uint64_t old_groups, uint32_t* err, cudaStream_t s) {
   if (old_groups == 0) return cudaSuccess;
-  int grid = (int)std::min<uint64_t>((old_groups + 255) / 256, 148 * 8);
+  int grid = (int)std::min<uint64_t>((old_groups + 255) / 256, grid_cap(8));
   agg_rehash_kernel<<<grid, 256, 0, s>>>(A, old_table, old_occ, old_groups, err);
   return cudaGetLastError();
 }
 cudaError_t launch_agg_migrate(const AggParams& A_new, const AggMigrateMap& M, const uint8_t* old_table, const uint32_t* old_occ, uint64_t old_groups, uint32_t* err, cudaStream_t s) {
   if (old_groups == 0) return cudaSuccess;
-  int grid = (int)std::min<uint64_t>((old_groups + 255) / 256, 148 * 8);
+  int grid = (int)std::min<uint64_t>((old_groups + 255) / 256, grid_cap(8));
   agg_migrate_kernel<<<grid, 256, 0, s>>>(A_new, M, old_table, old_occ, old_groups, err);
   return cudaGetLastError();
 }
 cudaError_t launch_agg_init_direct(const AggParams& A, cudaStream_t s) {
   const uint64_t n_entries = A.capacity_mask + 2;
   const uint64_t words = n_entries * A.entry_words;
-  agg_init_direct_kernel<<<(int)std::min<uint64_t>((words + 255) / 256, 148 * 16), 256, 0, s>>>(A, n_entries);
+  agg_init_direct_kernel<<<(int)std::min<uint64_t>((words + 255) / 256, grid_cap(16)), 256, 0, s>>>(A, n_entries);
   return cudaGetLastError();
 }
 cudaError_t launch_agg_build_occ(const AggParams& A, unsigned long long* counter, cudaStream_t s) {
   const uint64_t n_entries = A.capacity_mask + 2;
-  agg_build_occ_kernel<<<(int)std::min<uint64_t>((n_entries + 255) / 256, 148 * 16), 256, 0, s>>>(A, counter);
+  agg_build_occ_kernel<<<(int)std::min<uint64_t>((n_entries + 255) / 256, grid_cap(16)), 256, 0, s>>>(A, counter);
   return cudaGetLastError();
 }
 cudaError_t launch_agg_extract(const AggParams& A, const AggExtractParams& X, uint64_t n_groups, uint32_t* err, cudaStream_t s) {
   if (n_groups == 0) return cudaSuccess;
-  int grid = (int)std::min<uint64_t>((n_groups + 255) / 256, 148 * 8);
+  int grid = (int)std::min<uint64_t>((n_groups + 255) / 256, grid_cap(8));
   agg_extract_kernel<<<grid, 256, 0, s>>>(A, X, n_groups, err);
   return cudaGetLastError();
 }
@@ -2181,30 +2181,30 @@ __global__ void u32_to_bytes_kernel(const uint32_t* __restrict__ in, uint8_t* __
 }
 cudaError_t launch_u32_to_bytes(const uint32_t* in, uint8_t* out, int64_t n, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
-  u32_to_bytes_kernel<<<(int)std::min<int64_t>((n + 255) / 256, 148 * 8), 256, 0, s>>>(in, out, n);
+  u32_to_bytes_kernel<<<(int)std::min<int64_t>((n + 255) / 256, grid_cap(8)), 256, 0, s>>>(in, out, n);
   return cudaGetLastError();
 }
 cudaError_t launch_pack_bytes(const uint8_t* bytes, uint32_t* bits, int64_t n, unsigned long long* null_count, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
-  int grid = (int)std::min<int64_t>((n + 255) / 256, 148 * 8);
+  int grid = (int)std::min<int64_t>((n + 255) / 256, grid_cap(8));
   pack_bytes_kernel<<<grid, 256, 0, s>>>(bytes, bits, n, null_count);
   return cudaGetLastError();
 }
 cudaError_t launch_unpack_bits(const uint8_t* bits, uint8_t* bytes, int64_t n, int64_t bit_offset, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
-  int grid = (int)std::min<int64_t>((n + 255) / 256, 148 * 8);
+  int grid = (int)std::min<int64_t>((n + 255) / 256, grid_cap(8));
   unpack_bits_kernel<<<grid, 256, 0, s>>>(bits, bytes, n, bit_offset);
   return cudaGetLastError();
 }
 cudaError_t launch_resolve_views(void* views, int64_t n, const uint64_t* bases, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
-  int grid = (int)std::min<int64_t>((n + 255) / 256, 148 * 8);
+  int grid = (int)std::min<int64_t>((n + 255) / 256, grid_cap(8));
   resolve_views_kernel<<<grid, 256, 0, s>>>(reinterpret_cast<ulonglong2*>(views), n, bases);
   return cudaGetLastError();
 }
 cudaError_t launch_utf8_to_views(const int32_t* offsets, const uint8_t* bytes, void* views, int64_t n, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
-  int grid = (int)std::min<int64_t>((n + 255) / 256, 148 * 8);
+  int grid = (int)std::min<int64_t>((n + 255) / 256, grid_cap(8));
   utf8_to_views_kernel<<<grid, 256, 0, s>>>(offsets, bytes, reinterpret_cast<ulonglong2*>(views), n);
   return cudaGetLastError();
 }
@@ -2230,19 +2230,19 @@ cudaError_t launch_exclusive_scan_u32(const uint32_t* in, int64_t n, uint64_t* o
 }
 cudaError_t launch_view_lengths(const void* views, int64_t n, uint32_t* lens, int all, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
-  int grid = (int)std::min<int64_t>((n + 255) / 256, 148 * 8);
+  int grid = (int)std::min<int64_t>((n + 255) / 256, grid_cap(8));
   view_long_lengths_kernel<<<grid, 256, 0, s>>>(reinterpret_cast<const ulonglong2*>(views), n, lens, all);
   return cudaGetLastError();
 }
 cudaError_t launch_views_to_arrow(void* views, int64_t n, const uint64_t* offs, uint8_t* heap, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
-  int grid = (int)std::min<int64_t>((n + 255) / 256, 148 * 8);
+  int grid = (int)std::min<int64_t>((n + 255) / 256, grid_cap(8));
   views_to_arrow_kernel<<<grid, 256, 0, s>>>(reinterpret_cast<ulonglong2*>(views), n, offs, heap);
   return cudaGetLastError();
 }
 cudaError_t launch_views_to_utf8(const void* views, int64_t n, const uint64_t* offs, int32_t* out_offsets, uint8_t* heap, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
-  int grid = (int)std::min<int64_t>((n + 255) / 256, 148 * 8);
+  int grid = (int)std::min<int64_t>((n + 255) / 256, grid_cap(8));
   views_to_utf8_kernel<<<grid, 256, 0, s>>>(reinterpret_cast<const ulonglong2*>(views), n, offs, out_offsets, heap);
   return cudaGetLastError();
 }

@@ -91,7 +91,7 @@ __global__ void join_multi_kernel(JoinMultiParams P) {
 
 cudaError_t launch_join_multi(const JoinMultiParams& P, cudaStream_t s) {
   if (P.n_probe == 0) return cudaSuccess;
-  int grid = (int)std::min<int64_t>((P.n_probe + 255) / 256, 148 * 16);
+  int grid = (int)std::min<int64_t>((P.n_probe + 255) / 256, grid_cap(16));
   join_multi_kernel<<<grid, 256, 0, s>>>(P);
   return cudaGetLastError();
 }
@@ -111,7 +111,7 @@ __global__ void gather_rows_kernel(const uint8_t* __restrict__ src, uint8_t* __r
 }
 cudaError_t launch_gather_rows(const uint8_t* src, uint8_t* dst, const int64_t* idx, int64_t n, int width, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
-  int grid = (int)std::min<int64_t>((n + 255) / 256, 148 * 16);
+  int grid = (int)std::min<int64_t>((n + 255) / 256, grid_cap(16));
   gather_rows_kernel<<<grid, 256, 0, s>>>(src, dst, idx, n, width);
   return cudaGetLastError();
 }
@@ -124,7 +124,7 @@ __global__ void gather_bits_kernel(const uint8_t* __restrict__ bits, uint8_t* __
 }
 cudaError_t launch_gather_bits(const uint8_t* bits, uint8_t* out, const int64_t* idx, int64_t n, int dflt, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
-  int grid = (int)std::min<int64_t>((n + 255) / 256, 148 * 16);
+  int grid = (int)std::min<int64_t>((n + 255) / 256, grid_cap(16));
   gather_bits_kernel<<<grid, 256, 0, s>>>(bits, out, idx, n, dflt);
   return cudaGetLastError();
 }
@@ -146,7 +146,7 @@ __global__ void max_view_len_kernel(const ulonglong2* views, int64_t n, unsigned
 }
 cudaError_t launch_max_view_len(const void* views, int64_t n, unsigned int* out, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
-  int grid = (int)std::min<int64_t>((n + 255) / 256, 148 * 8);
+  int grid = (int)std::min<int64_t>((n + 255) / 256, grid_cap(8));
   max_view_len_kernel<<<grid, 256, 0, s>>>(reinterpret_cast<const ulonglong2*>(views), n, out);
   return cudaGetLastError();
 }
@@ -213,7 +213,7 @@ __global__ void sort_encode_kernel(SortEncodeParams P) {
 }
 cudaError_t launch_sort_encode(const SortEncodeParams& P, cudaStream_t s) {
   if (P.n == 0) return cudaSuccess;
-  int grid = (int)std::min<int64_t>((P.n + 255) / 256, 148 * 8);
+  int grid = (int)std::min<int64_t>((P.n + 255) / 256, grid_cap(8));
   sort_encode_kernel<<<grid, 256, (size_t)P.key_bytes * 8, s>>>(P);
   return cudaGetLastError();
 }
@@ -313,7 +313,7 @@ cudaError_t radix_sort_indices(const uint8_t* keys, int key_bytes, int64_t n, co
   auto trivial = [&](int d) { return (hb[(size_t)d] & hb[(size_t)key_bytes + d] & 0xFFu) == 0; };
   const int64_t n_chunks = (n + RADIX_CHUNK - 1) / RADIX_CHUNK;
   const int blocks = (int)((n_chunks + 7) / 8);
-  const int flat = (int)std::min<int64_t>((n + 255) / 256, 148 * 8);
+  const int flat = (int)std::min<int64_t>((n + 255) / 256, grid_cap(8));
   const uint32_t* in_idx = nullptr;            // nullptr = identity order
   uint32_t* out_idx = S.idx_a;
   uint64_t* kw_in = S.kw_a; uint64_t* kw_out = S.kw_b;
@@ -383,11 +383,11 @@ __global__ void topk_compact_kernel(const uint8_t* __restrict__ keys, int key_by
   }
 }
 cudaError_t launch_topk_hist(const uint8_t* keys, int key_bytes, int64_t n, int used, uint64_t prefix, int digit_bits, uint32_t* hist, cudaStream_t s) {
-  topk_hist_kernel<<<(int)std::min<int64_t>((n + 255) / 256, 148 * 8), 256, 0, s>>>(keys, key_bytes, n, used, prefix, digit_bits, hist);
+  topk_hist_kernel<<<(int)std::min<int64_t>((n + 255) / 256, grid_cap(8)), 256, 0, s>>>(keys, key_bytes, n, used, prefix, digit_bits, hist);
   return cudaGetLastError();
 }
 cudaError_t launch_topk_compact(const uint8_t* keys, int key_bytes, int64_t n, int used, uint64_t threshold, int64_t* out, unsigned long long* counter, cudaStream_t s) {
-  topk_compact_kernel<<<(int)std::min<int64_t>((n + 255) / 256, 148 * 8), 256, 0, s>>>(keys, key_bytes, n, used, threshold, out, counter);
+  topk_compact_kernel<<<(int)std::min<int64_t>((n + 255) / 256, grid_cap(8)), 256, 0, s>>>(keys, key_bytes, n, used, threshold, out, counter);
   return cudaGetLastError();
 }
 
@@ -421,7 +421,7 @@ __global__ void merge_rank_kernel(const uint8_t* __restrict__ keys, int key_byte
 }
 cudaError_t launch_merge_rank(const uint8_t* keys, int key_bytes, const int64_t* run_off, int n_runs, int64_t n, int64_t* perm, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
-  merge_rank_kernel<<<(int)std::min<int64_t>((n + 255) / 256, 148 * 8), 256, 0, s>>>(keys, key_bytes, run_off, n_runs, n, perm);
+  merge_rank_kernel<<<(int)std::min<int64_t>((n + 255) / 256, grid_cap(8)), 256, 0, s>>>(keys, key_bytes, run_off, n_runs, n, perm);
   return cudaGetLastError();
 }
 
@@ -441,7 +441,7 @@ __global__ void key_hash_kernel(const uint8_t* __restrict__ keys, int key_bytes,
 }
 cudaError_t launch_key_hash(const uint8_t* keys, int key_bytes, int64_t n, uint8_t* out8, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
-  key_hash_kernel<<<(int)std::min<int64_t>((n + 255) / 256, 148 * 8), 256, 0, s>>>(keys, key_bytes, n, out8);
+  key_hash_kernel<<<(int)std::min<int64_t>((n + 255) / 256, grid_cap(8)), 256, 0, s>>>(keys, key_bytes, n, out8);
   return cudaGetLastError();
 }
 __global__ void group_heads_kernel(const uint8_t* __restrict__ keys, int key_bytes, const uint32_t* __restrict__ idx, int64_t n, uint32_t* __restrict__ heads,
@@ -458,7 +458,7 @@ __global__ void group_heads_kernel(const uint8_t* __restrict__ keys, int key_byt
 cudaError_t launch_group_heads(const uint8_t* keys, int key_bytes, const uint32_t* idx, int64_t n, uint32_t* heads, const uint8_t* hashes,
                                unsigned long long* collisions, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
-  group_heads_kernel<<<(int)std::min<int64_t>((n + 255) / 256, 148 * 8), 256, 0, s>>>(keys, key_bytes, idx, n, heads, hashes, collisions);
+  group_heads_kernel<<<(int)std::min<int64_t>((n + 255) / 256, grid_cap(8)), 256, 0, s>>>(keys, key_bytes, idx, n, heads, hashes, collisions);
   return cudaGetLastError();
 }
 // group number of every input row (dense, in key order) and one representative input row per group
@@ -472,13 +472,13 @@ __global__ void assign_groups_kernel(const uint32_t* __restrict__ idx, const uin
 }
 cudaError_t launch_assign_groups(const uint32_t* idx, const uint32_t* heads, const uint64_t* before, int64_t n, int64_t* gid_of_row, int64_t* rep, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
-  assign_groups_kernel<<<(int)std::min<int64_t>((n + 255) / 256, 148 * 8), 256, 0, s>>>(idx, heads, before, n, gid_of_row, rep);
+  assign_groups_kernel<<<(int)std::min<int64_t>((n + 255) / 256, grid_cap(8)), 256, 0, s>>>(idx, heads, before, n, gid_of_row, rep);
   return cudaGetLastError();
 }
 
 cudaError_t launch_iota(int64_t* out, int64_t n, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
-  iota_kernel<<<(int)std::min<int64_t>((n + 255) / 256, 148 * 8), 256, 0, s>>>(out, n);
+  iota_kernel<<<(int)std::min<int64_t>((n + 255) / 256, grid_cap(8)), 256, 0, s>>>(out, n);
   return cudaGetLastError();
 }
 __global__ void iota_stride_kernel(int64_t* out, int64_t first, int64_t stride, int64_t n) {
@@ -486,12 +486,12 @@ __global__ void iota_stride_kernel(int64_t* out, int64_t first, int64_t stride, 
 }
 cudaError_t launch_iota_stride(int64_t* out, int64_t first, int64_t stride, int64_t n, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
-  iota_stride_kernel<<<(int)std::min<int64_t>((n + 255) / 256, 148 * 8), 256, 0, s>>>(out, first, stride, n);
+  iota_stride_kernel<<<(int)std::min<int64_t>((n + 255) / 256, grid_cap(8)), 256, 0, s>>>(out, first, stride, n);
   return cudaGetLastError();
 }
 cudaError_t launch_widen_u32(const uint32_t* in, int64_t* out, int64_t n, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
-  widen_u32_kernel<<<(int)std::min<int64_t>((n + 255) / 256, 148 * 8), 256, 0, s>>>(in, out, n);
+  widen_u32_kernel<<<(int)std::min<int64_t>((n + 255) / 256, grid_cap(8)), 256, 0, s>>>(in, out, n);
   return cudaGetLastError();
 }
 
@@ -504,7 +504,7 @@ __global__ void rebase_views_kernel(ulonglong2* views, int64_t n, uint64_t heap_
 }
 cudaError_t launch_rebase_views(void* views, int64_t n, uint64_t heap_base, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
-  rebase_views_kernel<<<(int)std::min<int64_t>((n + 255) / 256, 148 * 8), 256, 0, s>>>(reinterpret_cast<ulonglong2*>(views), n, heap_base);
+  rebase_views_kernel<<<(int)std::min<int64_t>((n + 255) / 256, grid_cap(8)), 256, 0, s>>>(reinterpret_cast<ulonglong2*>(views), n, heap_base);
   return cudaGetLastError();
 }
 
@@ -516,7 +516,7 @@ __global__ void multi_copy_kernel(const CopySeg* __restrict__ segs, int n) {
 }
 cudaError_t launch_multi_copy_raw(const CopySeg* dev_segs, int n, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
-  multi_copy_kernel<<<std::min(n, 148 * 4), 256, 0, s>>>(dev_segs, n);
+  multi_copy_kernel<<<std::min(n, grid_cap(4)), 256, 0, s>>>(dev_segs, n);
   return cudaGetLastError();
 }
 

@@ -158,7 +158,7 @@ struct AggParams {
   // Direct-key protocol (tables whose packed key is ONE 8-byte word: a single integer / date / narrow-decimal / float key that is
   // never null).  Every entry is pre-initialised to [0, 0, DIRECT_EMPTY_KEY, accumulator identities]; a slot is claimed by ONE
   // 64-bit compare-and-swap on its key word -- no state word, no lock, no release fence, no acquire loads (the fence and the
-  // counter round trip were 60 % of the 15 M-group aggregation's stall samples, profiles/r02_agg_highcard_*).  The one key equal
+  // counter round trip are most of a 15 M-group aggregation's stall samples).  The one key equal
   // to the sentinel lives in an extra entry behind the table.  `occ` is built by a scan before extraction / re-hashing.
   int32_t direct_key;
   // Bounded table: the table is sized for the groups the operator expects, not for its input rows.  A CTA that sees

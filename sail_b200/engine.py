@@ -8,7 +8,7 @@ bench: `GpuExec` <-> a DataFusion `ExecutionPlan` node, `push/finish/pull` <-> w
 through `include/sailgpu.h` entry points with Arrow C Data Interface structs -- no torch types.
 
 There is no CPU fallback: importing works anywhere (so symbol/ABI tests run on CPU), but creating a
-`Context` without a B200 raises `GpuUnavailable`.
+`Context` without an H100 raises `GpuUnavailable`.
 """
 from __future__ import annotations
 

@@ -1,5 +1,5 @@
 """Plan-time kernel specialisation for the pipelines bench.py and the evidence scripts run: generates and NVRTC-compiles
-their specialised kernels into sail_b200/_build/jit_cache (no GPU needed), so that the first batch on the GPU box finds
+their specialised kernels into sail_b200/_build/jit_cache (no GPU needed), so that the first batch on the GPU finds
 the cubin instead of paying a compilation.  What a rewrite pass does through sailgpu_jit_precompile while planning."""
 from __future__ import annotations
 

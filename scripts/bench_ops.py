@@ -1,4 +1,4 @@
-"""Per-operator throughput on one B200 (inputs resident in HBM), with the algorithmic-bytes formulas of SURVEY.md
+"""Per-operator throughput on one H100 (inputs resident in HBM), with the algorithmic-bytes formulas of SURVEY.md
 section 8(d) and the measured HBM peak: FilterExec, ProjectionExec, AggregateExec (low / high cardinality), HashJoinExec
 (build + probe), SortExec, hash RepartitionExec.  Times are CUDA-synchronised wall clock around push/finish/pull_device
 of ONE operator (device hand-off on both sides), best of `reps`."""
@@ -53,7 +53,7 @@ def run(ctx, spec, inputs, reps=3):
 
 def main():
     sf = float(sys.argv[1]) if len(sys.argv) > 1 else 10.0
-    peak = 6489.6
+    peak = 3350.0       # H100 SXM data sheet (HBM3), used when no measured peak is present
     pk = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(pk):
         peak = float(json.load(open(pk))["hbm_gbs"])

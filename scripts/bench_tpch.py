@@ -1,4 +1,4 @@
-"""All 22 TPC-H queries on one B200 with the referenced columns resident in HBM: wall-clock per query through the C ABI (every
+"""All 22 TPC-H queries on one H100 with the referenced columns resident in HBM: wall-clock per query through the C ABI (every
 intermediate stays on the device), rows/s over the scanned rows, per-operator times, and the total of the 22 (SURVEY.md section 8d:
 "total 22-query wall-clock").  Result parity of every plan is the test-suite's job (golden snapshot at SF0.001, oracle at SF0.1).
 Usage: python scripts/bench_tpch.py [SF] [reps]"""

@@ -1,4 +1,4 @@
-"""ClickBench on one B200: every query of sail_b200/clickbench.py through the C ABI, (1) checked against the SQL restated in pandas
+"""ClickBench on one H100: every query of sail_b200/clickbench.py through the C ABI, (1) checked against the SQL restated in pandas
 (tests/clickbench_sql.py) on a small synthetic hits table, (2) timed on a larger one resident in HBM.  One JSON line per query and
 leg is appended to --out as soon as it is known, and a query is marked "started" before it runs, so that a crash costs one
 query: run again with the same --out and the finished (or crashed) ones are skipped.

@@ -1,5 +1,5 @@
-"""Where does the first run of a high-cardinality aggregate spend its time?  ClickBench [04] (count(DISTINCT UserID)) on 3 M rows took
-22 s on its first run and 1 ms afterwards (profiles/r02_clickbench_gpu.jsonl).  Prints per-operator wall time of the first runs.
+"""Where does the first run of a high-cardinality aggregate spend its time?  ClickBench [04] (count(DISTINCT UserID)) on 3 M rows was
+far slower on its first run than afterwards.  Prints per-operator wall time of the first runs.
 
     SAILGPU_JIT_VERBOSE=1 python scripts/first_run_probe.py [rows]
 """

@@ -1,9 +1,9 @@
 """NVRTC-compiles the specialised kernel of every Filter / Projection / Aggregate node of the ClickBench (and, with --tpch, the
-TPC-H) plans for sm_100a -- no GPU needed -- into a SCRATCH cache (never the shipped one: a cached cubin is used from the first
+TPC-H) plans for sm_90a -- no GPU needed -- into a SCRATCH cache (never the shipped one: a cached cubin is used from the first
 batch on, and only the bench pipelines' kernels are parity-checked at that size), and prints one line per kernel with its
 resource usage.  What `sailgpu_jit_precompile(.., SAILGPU_JIT_COMPILE)` would do for a rewrite pass at plan time.
 
-    python scripts/jit_compile_all.py [--tpch] > profiles/r02_jit_clickbench_compile.txt
+    python scripts/jit_compile_all.py [--tpch]
 """
 import json
 import os
@@ -65,7 +65,7 @@ def main():
         return out
     for name, plan, _ in work:
         walk(plan, name)
-    print(f"# {ok} kernels compiled for sm_100a, {refused} pipelines stay interpreted, {time.time() - t0:.0f} s on the CPU (NVRTC)")
+    print(f"# {ok} kernels compiled for sm_90a, {refused} pipelines stay interpreted, {time.time() - t0:.0f} s on the CPU (NVRTC)")
 
 
 if __name__ == "__main__":

@@ -1,4 +1,4 @@
-//! sail-gpu -- B200 execution of Sail's physical-plan hot path behind DataFusion's `ExecutionPlan`.
+//! sail-gpu -- H100 execution of Sail's physical-plan hot path behind DataFusion's `ExecutionPlan`.
 //!
 //! NOT COMPILED in this repository (the build image has no Rust toolchain); see shim/README.md.
 //!

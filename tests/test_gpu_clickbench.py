@@ -1,7 +1,7 @@
 """ClickBench (BASELINE.json configs[4]) on the GPU: the 37 plans of sail_b200/clickbench.py through the C ABI on a synthetic hits
 table, each result checked against the query's SQL restated in pandas (tests/clickbench_sql.py) -- up to ties for ORDER BY ..
 LIMIT, Float64 AVG within 1e-6 relative, everything else bit-exact.  The same check runs the oracle on the CPU
-(tests/test_clickbench.py).  Evidence of the first run, with per-query times on a 3 M-row table: profiles/r02_clickbench_gpu.jsonl."""
+(tests/test_clickbench.py)."""
 import numpy as np
 import pyarrow as pa
 import pytest

@@ -1,9 +1,8 @@
 """The kernel specialiser's code generator on the CPU: for every Filter / Projection / Aggregate node of the 22 TPC-H and the 37
 ClickBench plans `sailgpu_jit_precompile` (no device, no NVRTC: source only, nothing is written to the kernel cache) either
 emits the CUDA source of the specialised kernel or says why the pipeline stays interpreted (SAILGPU_ERR_UNSUPPORTED).
-NVRTC-compiling all of them for sm_100a takes a minute and is what `__graft_entry__.build()` does for the bench pipelines;
-`scripts/jit_compile_all.py` does it for every ClickBench pipeline into a scratch cache (profiles/r02_jit_clickbench_compile.txt: 152
-kernels, no compile error)."""
+NVRTC-compiling all of them for sm_90a takes a minute and is what `__graft_entry__.build()` does for the bench pipelines;
+`scripts/jit_compile_all.py` does it for every ClickBench pipeline into a scratch cache."""
 import json
 
 import pytest
