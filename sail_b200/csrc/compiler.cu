@@ -464,7 +464,8 @@ void PipelineCompiler::finalize(CompiledPipeline& out, Ctx* ctx, int hot_wanted)
   };
   const int force_rpt = env_int("SAILGPU_RPT", 0), force_stages = env_int("SAILGPU_STAGES", 0), force_hot = env_int("SAILGPU_HOT", -1);
   // (rows per thread, input stages) in order of preference, as swept with scripts/sweep_q1.py and scripts/bench_ops.py (the
-  // order was tuned before the move to H100 and has not been swept there again):
+  // interpreter's order was tuned before the move to H100; the specialised kernel's stage count -- jit.cu: jit_plan -- was
+  // measured on H100, DESIGN.md section 4.1):
   // aggregation wants 2 CTAs/SM of 512-row tiles; plain projection streams best with big double-buffered tiles;
   // compaction / join / partition sinks prefer big single-stage tiles and more resident CTAs
   static const int C_AGG[][2] = {{2, 1}, {1, 2}, {2, 2}, {1, 1}, {4, 1}, {4, 2}};

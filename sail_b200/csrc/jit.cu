@@ -435,18 +435,20 @@ bool jit_plan(const CompiledPipeline& cp, size_t max_smem, JitPlan* plan) {
   uint32_t stage = 0;
   for (auto& r : J.inputs) stage += align128(r.width ? (uint32_t)r.width * tile : tile / 8);
   p.stage_bytes = stage;
-  int target = 3, cap = p.rpt >= 4 ? 2 : 3;
+  int target = 3, cap = p.rpt >= 4 ? 2 : 3, max_s = 4;
   if (cp.sink == SINK_AGG) {
     const AggParams& A = J.agg;
     const int tier = A.cold_only ? 0 : A.reg_path ? 2 : A.hot_groups > 0 ? 1 : 0;
     const int hot_g = std::min(8, std::max(A.hot_groups, tier == 2 ? REG_GROUPS : 0));
     if (tier > 0) p.scratch_bytes = align128((uint32_t)(32 + hot_g * (HOT_KEY_WORDS * 8 + 8) + (NT / 32) * hot_g * (1 + 2 * A.n_accs) * 8));
     target = tier == 0 ? 3 : 2; cap = tier == 0 ? 4 : 2;
+    // dictionary / register tiers: two stages streamed faster than three or four on H100 (DESIGN.md section 4.1)
+    if (tier > 0) max_s = 2;
   }
   const int force_s = env_i("SAILGPU_JIT_STAGES", 0);
   int chosen = 0;
   for (int s = 4; s >= 2 && !chosen; --s) {
-    if (force_s && s != force_s) continue;
+    if (force_s ? s != force_s : s > max_s) continue;
     const size_t smem = JIT_HDR_BYTES + p.scratch_bytes + (size_t)s * stage;
     if (smem > max_smem) continue;
     const int ctas = (int)((228 * 1024) / (smem + 1024));
