@@ -36,6 +36,12 @@ int32_t guard(std::string* err, F&& f) {
   }
 }
 void set_device(const Ctx& c) { SG_CUDA(cudaSetDevice(c.device)); }
+// charges the stream drains of one call on an operator handle to that operator (a chain's handle gets those of its stages)
+struct SyncCharge {
+  sailgpu_op* h; uint64_t s0;
+  explicit SyncCharge(sailgpu_op* op) : h(op), s0(op->owner->ctx.host_syncs.load()) {}
+  ~SyncCharge() { if (h->op) h->op->m.host_syncs += h->owner->ctx.host_syncs.load() - s0; }
+};
 using CtxLock = std::lock_guard<std::recursive_mutex>;
 }  // namespace
 
@@ -94,6 +100,7 @@ SAILGPU_API void sailgpu_ctx_destroy(sailgpu_ctx* c) {
   c->ctx.shared_objects.clear();      // compiled pipelines and their literal buffers
   c->ctx.dead.store(true);
   if (c->ctx.stream) { cudaStreamSynchronize(c->ctx.stream); cudaStreamDestroy(c->ctx.stream); c->ctx.stream = nullptr; }
+  if (c->ctx.pinned_block) { cudaFreeHost(c->ctx.pinned_block); c->ctx.pinned_block = nullptr; }
   destroy_pack_pool(&c->ctx);
 }
 
@@ -120,7 +127,9 @@ SAILGPU_API int32_t sailgpu_op_create(sailgpu_ctx* c, const char* spec_json, siz
     for (int i = 0; i < n_inputs; ++i) ins.push_back(schema_from_arrow(input_schemas[i]));
     auto h = std::make_unique<sailgpu_op>();
     h->owner = c;
+    const uint64_t s0 = c->ctx.host_syncs.load();
     h->op = make_op(&c->ctx, spec, ins, partition);
+    h->op->m.host_syncs += c->ctx.host_syncs.load() - s0;
     h->input_finished.assign((size_t)n_inputs, false);
     schema_to_arrow(h->op->out_schema, out_schema);
     *out = h.release();
@@ -199,6 +208,7 @@ SAILGPU_API int32_t sailgpu_op_push(sailgpu_op* h, int32_t input_idx, struct Arr
   if (!h) return SAILGPU_ERR_INVALID;
   return guard(&h->last_error, [&] {
     CtxLock lk(h->owner->ctx.mu);
+    SyncCharge charge(h);
     set_device(h->owner->ctx);
     SG_CHECK(input_idx >= 0 && input_idx < (int)h->op->in_schemas.size(), SAILGPU_ERR_INVALID, "input index out of range");
     SG_CHECK(!h->input_finished[(size_t)input_idx], SAILGPU_ERR_STATE, "push after finish_input");
@@ -211,6 +221,7 @@ SAILGPU_API int32_t sailgpu_op_push_device(sailgpu_op* h, int32_t input_idx, str
   if (!h) return SAILGPU_ERR_INVALID;
   return guard(&h->last_error, [&] {
     CtxLock lk(h->owner->ctx.mu);
+    SyncCharge charge(h);
     set_device(h->owner->ctx);
     SG_CHECK(input_idx >= 0 && input_idx < (int)h->op->in_schemas.size(), SAILGPU_ERR_INVALID, "input index out of range");
     SG_CHECK(!h->input_finished[(size_t)input_idx], SAILGPU_ERR_STATE, "push after finish_input");
@@ -227,6 +238,7 @@ SAILGPU_API int32_t sailgpu_op_finish_input(sailgpu_op* h, int32_t input_idx) {
   if (!h) return SAILGPU_ERR_INVALID;
   return guard(&h->last_error, [&] {
     CtxLock lk(h->owner->ctx.mu);
+    SyncCharge charge(h);
     set_device(h->owner->ctx);
     SG_CHECK(input_idx >= 0 && input_idx < (int)h->op->in_schemas.size(), SAILGPU_ERR_INVALID, "input index out of range");
     if (h->input_finished[(size_t)input_idx]) return;
@@ -240,6 +252,7 @@ static int32_t pull_common(sailgpu_op* h, int part, struct ArrowArray* host_out,
   if (!h) return SAILGPU_ERR_INVALID;
   return guard(&h->last_error, [&] {
     CtxLock lk(h->owner->ctx.mu);
+    SyncCharge charge(h);
     set_device(h->owner->ctx);
     SG_CHECK(has_more && (host_out || dev_out), SAILGPU_ERR_INVALID, "null argument");
     BatchPtr b;
@@ -294,7 +307,8 @@ SAILGPU_API int64_t sailgpu_op_metrics(sailgpu_op* h, char* json_buf, size_t cap
                    "\"elapsed_compute\":%llu,\"build_input_rows\":%llu,\"build_input_batches\":%llu,\"build_time\":%llu,"
                    "\"join_time\":%llu,\"gpu.kernel_launches\":%llu,\"gpu.h2d_bytes\":%llu,\"gpu.d2h_bytes\":%llu,"
                    "\"gpu.pipeline_launches\":%llu,\"gpu.jit_launches\":%llu,\"gpu.pipeline_kernel_ns\":%llu,"
-                   "\"gpu.exchange_sent_bytes\":%llu,\"gpu.exchange_recv_bytes\":%llu,\"gpu.exchange_ns\":%llu,\"gpu.exchange_calls\":%llu}",
+                   "\"gpu.exchange_sent_bytes\":%llu,\"gpu.exchange_recv_bytes\":%llu,\"gpu.exchange_ns\":%llu,\"gpu.exchange_calls\":%llu,"
+                   "\"gpu.host_syncs\":%llu}",
                    (unsigned long long)m.output_rows, (unsigned long long)m.output_batches, (unsigned long long)m.input_rows,
                    (unsigned long long)m.input_batches, (unsigned long long)m.elapsed_compute_ns, (unsigned long long)m.build_input_rows,
                    (unsigned long long)m.build_input_batches, (unsigned long long)m.build_time_ns, (unsigned long long)m.join_time_ns,
@@ -302,7 +316,7 @@ SAILGPU_API int64_t sailgpu_op_metrics(sailgpu_op* h, char* json_buf, size_t cap
                    (unsigned long long)h->owner->ctx.d2h_bytes.load(), (unsigned long long)h->op->m.pipeline_launches, (unsigned long long)h->op->m.jit_launches,
                    (unsigned long long)h->op->pipeline_kernel_ns(), (unsigned long long)h->owner->ctx.exch_sent_bytes.load(),
                    (unsigned long long)h->owner->ctx.exch_recv_bytes.load(), (unsigned long long)h->owner->ctx.exch_ns.load(),
-                   (unsigned long long)h->owner->ctx.exch_calls.load());
+                   (unsigned long long)h->owner->ctx.exch_calls.load(), (unsigned long long)m.host_syncs);
   if (json_buf && cap) { size_t k = std::min<size_t>((size_t)n, cap - 1); memcpy(json_buf, tmp, k); json_buf[k] = 0; }
   return n + 1;
 }

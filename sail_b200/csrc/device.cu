@@ -3,6 +3,7 @@
 // This is the boundary the Rust shim crosses per RecordBatch (arrow::ffi::to_ffi / from_ffi);
 // ownership rules follow SURVEY.md section 8b "Ownership": inputs are producer-owned until their
 // release callback runs; outputs are library-owned until the consumer calls release.
+#include <algorithm>
 #include <cstdlib>
 #include <cstring>
 
@@ -162,7 +163,7 @@ DevColumn import_column(ImportJob& J, const Field& f, const ArrowArray* a, const
         doffs = borrow(offs, (size_t)(a->length + 1) * 4);
         int32_t last = 0;
         if (a->length) SG_CUDA(cudaMemcpyAsync(&last, offs + a->length, 4, cudaMemcpyDeviceToHost, stream));
-        SG_CUDA(cudaStreamSynchronize(stream));
+        stream_sync(ctx);
         dbytes = borrow(bytes, (size_t)last);
       } else {
         doffs = J.upload(offs, a->length + 1, 4);
@@ -188,7 +189,7 @@ DevColumn import_column(ImportJob& J, const Field& f, const ArrowArray* a, const
       if (n_data > 0) {
         std::vector<int64_t> sizes((size_t)n_data);
         const int64_t* size_buf = static_cast<const int64_t*>(a->buffers[a->n_buffers - 1]);
-        if (on_device) { SG_CUDA(cudaMemcpyAsync(sizes.data(), size_buf, (size_t)n_data * 8, cudaMemcpyDeviceToHost, stream)); SG_CUDA(cudaStreamSynchronize(stream)); }
+        if (on_device) { SG_CUDA(cudaMemcpyAsync(sizes.data(), size_buf, (size_t)n_data * 8, cudaMemcpyDeviceToHost, stream)); stream_sync(ctx); }
         else std::memcpy(sizes.data(), size_buf, (size_t)n_data * 8);
         auto bases = std::make_shared<std::vector<uint64_t>>((size_t)n_data);
         for (int64_t k = 0; k < n_data; ++k) {
@@ -202,7 +203,7 @@ DevColumn import_column(ImportJob& J, const Field& f, const ArrowArray* a, const
         J.after([=] {
           SG_CUDA(cudaMemcpyAsync(dbases->ptr, bases->data(), (size_t)n_data * 8, cudaMemcpyHostToDevice, stream));
           SG_CUDA(launch_resolve_views(vdata->ptr, n, static_cast<const uint64_t*>(dbases->ptr), stream));
-          SG_CUDA(cudaStreamSynchronize(stream));   // `bases` is host memory owned by this closure
+          stream_sync(ctx);   // `bases` is host memory owned by this closure
         });
         c.heaps.push_back(dbases);
       }
@@ -296,11 +297,17 @@ void init_array(ArrowArray* a, int64_t length, int64_t null_count, ArrayPriv* p)
 
 // strings: produce Arrow-conformant buffers on the device from resolved views
 struct StringExport { BufPtr views_or_offsets, heap; int64_t heap_bytes = 0; };
-StringExport export_strings(Ctx* ctx, const DevColumn& c, bool as_utf8) {
+// `inline_known`: the caller has established that every view of the column is inline (<= 12 bytes)
+StringExport export_strings(Ctx* ctx, const DevColumn& c, bool as_utf8, bool inline_known) {
   StringExport out;
   const int64_t n = c.length;
   if (n == 0) {
     out.views_or_offsets = dev_alloc_zero(ctx, as_utf8 ? 4 : 0);
+    out.heap = dev_alloc(ctx, 0);
+    return out;
+  }
+  if (inline_known) {
+    out.views_or_offsets = c.data;
     out.heap = dev_alloc(ctx, 0);
     return out;
   }
@@ -310,7 +317,7 @@ StringExport export_strings(Ctx* ctx, const DevColumn& c, bool as_utf8) {
     unsigned int max_len = 0;
     SG_CUDA(launch_max_view_len(c.data->ptr, n, static_cast<unsigned int*>(mx->ptr), ctx->stream));
     SG_CUDA(cudaMemcpyAsync(&max_len, mx->ptr, 4, cudaMemcpyDeviceToHost, ctx->stream));
-    SG_CUDA(cudaStreamSynchronize(ctx->stream));
+    stream_sync(ctx);
     if (max_len <= 12) {
       out.views_or_offsets = c.data;
       out.heap = dev_alloc(ctx, 0);
@@ -325,7 +332,7 @@ StringExport export_strings(Ctx* ctx, const DevColumn& c, bool as_utf8) {
   const int64_t nblocks = std::min<int64_t>(1024, (n + 4095) / 4096);
   uint64_t total = 0;
   SG_CUDA(cudaMemcpyAsync(&total, static_cast<uint64_t*>(scratch->ptr) + nblocks, 8, cudaMemcpyDeviceToHost, ctx->stream));
-  SG_CUDA(cudaStreamSynchronize(ctx->stream));
+  stream_sync(ctx);
   out.heap_bytes = (int64_t)total;
   out.heap = dev_alloc(ctx, (size_t)total);
   if (as_utf8) {
@@ -369,7 +376,7 @@ void finish_small_d2h(Ctx* ctx) {
   ctx->d2h_used = 0;
 }
 
-void export_column(Ctx* ctx, const Field& f, const DevColumn& c, ArrowArray* out, bool to_device) {
+void export_column(Ctx* ctx, const Field& f, const DevColumn& c, ArrowArray* out, bool to_device, bool inline_known = false) {
   auto* p = new ArrayPriv();
   const int64_t n = c.length;
   auto emit = [&](const BufPtr& b, size_t bytes) -> const void* {
@@ -381,7 +388,7 @@ void export_column(Ctx* ctx, const Field& f, const DevColumn& c, ArrowArray* out
   p->buffers.push_back(c.validity ? emit(c.validity, (size_t)((n + 7) / 8)) : nullptr);
   if (f.type.is_string()) {
     const bool as_utf8 = f.type.id == TypeId::Utf8;
-    StringExport s = export_strings(ctx, c, as_utf8);
+    StringExport s = export_strings(ctx, c, as_utf8, inline_known);
     if (as_utf8) {
       p->buffers.push_back(emit(s.views_or_offsets, (size_t)(n + 1) * 4));
       p->buffers.push_back(emit(s.heap, (size_t)s.heap_bytes));
@@ -412,19 +419,45 @@ void export_column(Ctx* ctx, const Field& f, const DevColumn& c, ArrowArray* out
 
 }  // namespace
 
+// One synchronisation per batch: every Utf8View column is first exported as if all its strings were inline (its views are
+// then the Arrow views), with the longest length of each such column read back together with the data.  Only a column that
+// really holds longer strings is exported a second time, through the heap.
 void export_host_batch(Ctx* ctx, const Schema& schema, const BatchPtr& b, ArrowArray* out) {
   ctx->d2h_pending.clear(); ctx->d2h_used = 0;      // leftovers of an export that failed half way
   auto* p = new ArrayPriv();
   p->buffers.push_back(nullptr);
   p->children.resize(schema.size());
   p->child_ptrs.resize(schema.size());
+  std::vector<size_t> view_cols;
+  for (size_t i = 0; i < schema.size(); ++i)
+    if (schema[i].type.id == TypeId::Utf8View && b->cols[i].length > 0) view_cols.push_back(i);
+  const unsigned int* max_len = nullptr;
+  if (!view_cols.empty()) {
+    BufPtr mx = dev_alloc_zero(ctx, view_cols.size() * 4);
+    for (size_t k = 0; k < view_cols.size(); ++k)
+      SG_CUDA(launch_max_view_len(b->cols[view_cols[k]].data->ptr, b->cols[view_cols[k]].length, static_cast<unsigned int*>(mx->ptr) + k, ctx->stream));
+    max_len = static_cast<const unsigned int*>(to_host(ctx, mx->ptr, view_cols.size() * 4, p));
+  }
+  auto is_view = [&](size_t i) { return std::find(view_cols.begin(), view_cols.end(), i) != view_cols.end(); };
   for (size_t i = 0; i < schema.size(); ++i) {
     p->children[i].release = nullptr;
-    export_column(ctx, schema[i], b->cols[i], &p->children[i], false);
+    export_column(ctx, schema[i], b->cols[i], &p->children[i], false, is_view(i));
     p->child_ptrs[i] = &p->children[i];
   }
-  SG_CUDA(cudaStreamSynchronize(ctx->stream));
+  stream_sync(ctx);
   finish_small_d2h(ctx);
+  bool again = false;
+  for (size_t k = 0; k < view_cols.size(); ++k) {
+    if (max_len[k] <= 12) continue;
+    const size_t i = view_cols[k];
+    p->children[i].release(&p->children[i]);
+    export_column(ctx, schema[i], b->cols[i], &p->children[i], false, false);
+    again = true;
+  }
+  if (again) {
+    stream_sync(ctx);
+    finish_small_d2h(ctx);
+  }
   init_array(out, b->rows, 0, p);
   out->n_children = (int64_t)schema.size();
   out->children = p->child_ptrs.data();
@@ -450,7 +483,7 @@ void export_device_batch(Ctx* ctx, const Schema& schema, const BatchPtr& b, Arro
       export_column(ctx, schema[i], b->cols[i], &p->children[i], true);
       p->child_ptrs[i] = &p->children[i];
     }
-    SG_CUDA(cudaStreamSynchronize(ctx->stream));   // consumer may use any stream: hand over completed data
+    stream_sync(ctx);   // consumer may use any stream: hand over completed data
     init_array(&out->array, b->rows, 0, p);
     out->array.n_children = (int64_t)schema.size();
     out->array.children = p->child_ptrs.data();

@@ -63,7 +63,39 @@ struct Ctx {
   size_t cached_bytes = 0;
   static constexpr size_t CACHE_LIMIT = 64ull << 30;
   static size_t size_class(size_t padded) { return padded <= (1u << 20) ? (padded + 511) & ~(size_t)511 : (padded + (1u << 20) - 1) & ~(size_t)((1u << 20) - 1); }
+  // times the host waited for `stream` to drain (stream_sync); capi.cu charges each call's share to the operator it served
+  std::atomic<uint64_t> host_syncs{0};
+  // pinned 128-byte slots for the asynchronous read-backs of operators (pinned_slot_acquire / release): one block per context,
+  // because pinning memory per operator would cost more than the round trips it saves
+  static constexpr size_t PINNED_SLOT = 128, PINNED_SLOTS = 512;
+  void* pinned_block = nullptr;
+  std::vector<uint32_t> pinned_free;
+  uint32_t pinned_next = 0;
 };
+
+// Waits until everything queued on the context's stream has run.  Every such wait leaves the device without work until the
+// host queues more, so the library counts them (gpu.host_syncs).
+inline void stream_sync(Ctx* ctx) {
+  ctx->host_syncs++;
+  SG_CUDA(cudaStreamSynchronize(ctx->stream));
+}
+
+// A pinned, device-mapped host slot of Ctx::PINNED_SLOT bytes (kernels may write it through cudaHostGetDevicePointer); null
+// when pinning fails.
+inline void* pinned_slot_acquire(Ctx* ctx) {
+  if (!ctx->pinned_block) {
+    if (cudaHostAlloc(&ctx->pinned_block, Ctx::PINNED_SLOT * Ctx::PINNED_SLOTS, cudaHostAllocMapped) != cudaSuccess) { cudaGetLastError(); ctx->pinned_block = nullptr; return nullptr; }
+  }
+  uint32_t i;
+  if (!ctx->pinned_free.empty()) { i = ctx->pinned_free.back(); ctx->pinned_free.pop_back(); }
+  else if (ctx->pinned_next < Ctx::PINNED_SLOTS) i = ctx->pinned_next++;
+  else return nullptr;
+  return static_cast<uint8_t*>(ctx->pinned_block) + (size_t)i * Ctx::PINNED_SLOT;
+}
+inline void pinned_slot_release(Ctx* ctx, void* p) {
+  if (!p || !ctx->pinned_block) return;
+  ctx->pinned_free.push_back((uint32_t)((static_cast<uint8_t*>(p) - static_cast<uint8_t*>(ctx->pinned_block)) / Ctx::PINNED_SLOT));
+}
 
 // set by an atexit hook: CUDA may already be torn down when late destructors run at process exit
 extern std::atomic<bool> g_exiting;

@@ -7,6 +7,15 @@
 
 namespace sg {
 
+// Copies the first `words` words of an operator's scalars into mapped host memory and zeroes the hand-back counter of the next
+// launch: one tiny launch between two aggregate launches instead of a device->host copy and a memset.
+__global__ void agg_counters_kernel(const unsigned long long* __restrict__ scal, unsigned long long* host, int words, unsigned long long* zero) {
+  if (threadIdx.x < words) host[threadIdx.x] = scal[threadIdx.x];
+  __threadfence_system();
+  __syncthreads();
+  if (threadIdx.x == 0 && zero) *zero = 0;
+}
+
 
 // ------------------------------------------------------------------------------------------------
 // spec parsing
@@ -84,16 +93,21 @@ StageSpec parse_stage(const Json& j, const Schema& in, Schema* out) {
   return st;
 }
 
-void check_device_error(Ctx* ctx, uint32_t* dev_flag) {
-  uint32_t f = 0;
-  SG_CUDA(cudaMemcpyAsync(&f, dev_flag, 4, cudaMemcpyDeviceToHost, ctx->stream));
-  SG_CUDA(cudaStreamSynchronize(ctx->stream));
+// throws the error a kernel raised in `f` (the value of the device flag at `dev_flag`), after clearing the flag
+void raise_device_error(Ctx* ctx, uint32_t* dev_flag, uint32_t f) {
   if (!f) return;
   SG_CUDA(cudaMemsetAsync(dev_flag, 0, 4, ctx->stream));
   if (f & ERR_DIV_ZERO) fail(SAILGPU_ERR_ARITHMETIC, "Divide by zero");
   if (f & ERR_OVERFLOW) fail(SAILGPU_ERR_ARITHMETIC, "Arithmetic overflow");
   if (f & ERR_TABLE_FULL) fail(SAILGPU_ERR_CUDA, "hash table overflow");
   fail(SAILGPU_ERR_UNSUPPORTED, "unsupported value encountered on device");
+}
+
+void check_device_error(Ctx* ctx, uint32_t* dev_flag) {
+  uint32_t f = 0;
+  SG_CUDA(cudaMemcpyAsync(&f, dev_flag, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  stream_sync(ctx);
+  raise_device_error(ctx, dev_flag, f);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -231,7 +245,7 @@ struct PipelineOp : Op {
     SG_CUDA(launch_exclusive_scan_u32(static_cast<const uint32_t*>(counts->ptr), n_tiles + 1, static_cast<uint64_t*>(offs->ptr), static_cast<uint64_t*>(scratch->ptr), ctx->stream));
     unsigned long long total = 0;
     SG_CUDA(cudaMemcpyAsync(&total, static_cast<const uint64_t*>(offs->ptr) + n_tiles, 8, cudaMemcpyDeviceToHost, ctx->stream));
-    SG_CUDA(cudaStreamSynchronize(ctx->stream));
+    stream_sync(ctx);
     m.kernel_launches += 4;
     return run_streaming(sel_run, ctx, b2, m, nullptr, {}, static_cast<const unsigned long long*>(offs->ptr), (int64_t)total);
   }
@@ -244,26 +258,63 @@ struct PipelineOp : Op {
   // ---- aggregate ------------------------------------------------------------------------------
   // The group table is sized for the groups the operator expects, not for its input rows.  Every launch carries a group
   // limit (half the capacity minus what tiles in flight could still add); CTAs that see the table above it stop taking
-  // tiles and append the ones they still owned to a deferred list.  The host reads (groups, deferred) back at the next
-  // synchronisation point it needs anyway (next push / finish), and if tiles were handed back it grows the table by the
-  // observed groups-per-row ratio, rehashes, and re-launches over the list -- with the pipeline variant compiled for
+  // tiles and append the ones they still owned to a deferred list.  If tiles were handed back the host grows the table by
+  // the observed groups-per-row ratio, rehashes, and re-launches over the list -- with the pipeline variant compiled for
   // the global table alone when the input turned out to have many groups.
+  //
+  // Launches are pipelined one deep: after queueing the launch of batch k, the host queues an asynchronous copy of the
+  // counters (error flag, groups, both hand-back counts) into pinned memory and only then waits for the copy made after
+  // batch k-1.  The device already has batch k to work on, so that wait costs it nothing.  When k-1 handed nothing back
+  // and raised nothing, that is all.  Otherwise the host drains the stream and resolves k-1 and k together: a rehash
+  // or layout migration must never run on a group count older than the last launch.  Each of the two launches in
+  // flight has its own hand-back counter and list; the operator holds at most those two input batches.
   static constexpr uint64_t MIN_CAPACITY = 1ull << 22, MAX_CAPACITY = 1ull << 28;
   static constexpr uint64_t CARD_MANY_GROUPS = 256, HOT_GROUP_LIMIT = 1 << 16;
   static uint64_t min_capacity() { const char* v = getenv("SAILGPU_AGG_MIN_CAPACITY"); return v && *v ? next_pow2((uint64_t)atoll(v)) : MIN_CAPACITY; }
   bool use_cold = false;
   int64_t rows_in_table = 0;
-  int64_t known_groups = -1;      // group count read (and error flag checked) by the last resolve_pending(), -1 = stale
-  struct Pending { BatchPtr batch; std::shared_ptr<CompiledPipeline> cp; BufPtr deferred; int64_t n_tiles = 0; bool active = false; } pend;
+  int64_t known_groups = -1;      // group count read (and error flag checked) once nothing was in flight any more, -1 = stale
+  // a grouped launch whose hand-back has not been looked at yet; `slot` picks its hand-back counter and its counter copy
+  struct InFlight { BatchPtr batch; std::shared_ptr<CompiledPipeline> cp; BufPtr deferred; int slot = 0; };
+  std::deque<InFlight> inflight;
+  int next_slot = 0;
+  // what a counter copy holds: the first 56 bytes of the scalars (DevScalars: error @0, n_groups @24, hand-back counts @40, @48)
+  struct Counters { uint32_t error; uint32_t pad_[5]; unsigned long long n_groups, cursor, n_def[2]; };
+  static_assert(sizeof(Counters) == 56, "counter copy layout");
+  Counters* counters = nullptr;        // two copies, in a pinned slot of the context (or on the heap when pinning failed)
+  Counters* counters_dev = nullptr;    // the pinned slot as the device addresses it
+  bool counters_pinned = false, next_zeroed = false;
+  cudaEvent_t copied[2] = {nullptr, nullptr};
 
-  unsigned long long* n_deferred_ptr() { return reinterpret_cast<unsigned long long*>(static_cast<uint8_t*>(run.scal.buf->ptr) + 40); }
+  ~PipelineOp() override {
+    if (g_exiting.load()) return;
+    for (cudaEvent_t e : copied) if (e) cudaEventDestroy(e);
+    if (counters_pinned) pinned_slot_release(ctx, counters); else delete[] counters;
+  }
 
-  uint64_t read_n_groups() {
-    run.ensure_scratch();
-    unsigned long long g = 0;
-    SG_CUDA(cudaMemcpyAsync(&g, run.scal.n_groups(), 8, cudaMemcpyDeviceToHost, ctx->stream));
-    SG_CUDA(cudaStreamSynchronize(ctx->stream));
-    return g;
+  unsigned long long* n_deferred_ptr(int slot) { return reinterpret_cast<unsigned long long*>(static_cast<uint8_t*>(run.scal.buf->ptr) + 40 + 8 * slot); }
+
+  // queues the copy of the counters into copy `slot` and marks its completion; `zero_next`: also zero the hand-back counter of
+  // the other slot, which the next launch uses (launch_agg then skips its memset)
+  void copy_counters(int slot, bool zero_next) {
+    if (!counters) {
+      static_assert(2 * sizeof(Counters) <= Ctx::PINNED_SLOT, "pinned slot too small");
+      counters = static_cast<Counters*>(pinned_slot_acquire(ctx));
+      counters_pinned = counters != nullptr;
+      if (counters_pinned) SG_CUDA(cudaHostGetDevicePointer(reinterpret_cast<void**>(&counters_dev), counters, 0));
+      else counters = new Counters[2];
+      for (auto& e : copied) SG_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    }
+    if (counters_pinned) {
+      agg_counters_kernel<<<1, 32, 0, ctx->stream>>>(static_cast<const unsigned long long*>(run.scal.buf->ptr), reinterpret_cast<unsigned long long*>(&counters_dev[slot]),
+                                                     (int)(sizeof(Counters) / 8), zero_next ? n_deferred_ptr(slot ^ 1) : nullptr);
+      SG_CUDA(cudaGetLastError());
+      m.kernel_launches++;
+      next_zeroed = zero_next;
+    } else {
+      SG_CUDA(cudaMemcpyAsync(&counters[slot], run.scal.buf->ptr, sizeof(Counters), cudaMemcpyDeviceToHost, ctx->stream));
+    }
+    SG_CUDA(cudaEventRecord(copied[slot], ctx->stream));
   }
 
   void fill_table(AggParams& A) {
@@ -314,7 +365,7 @@ struct PipelineOp : Op {
   }
 
   // one launch over all tiles of `b` (list == null) or over the listed tiles; tiles handed back land in `deferred_out`
-  void launch_agg(const std::shared_ptr<CompiledPipeline>& cp, const DevBatch& b, const BufPtr& list, int64_t n_list, const BufPtr& deferred_out) {
+  void launch_agg(const std::shared_ptr<CompiledPipeline>& cp, const DevBatch& b, const BufPtr& list, int64_t n_list, const BufPtr& deferred_out, int slot) {
     PipelineParams P;
     run.prepare(P, *cp, b, 0, b.rows);
     if (list) { P.tile_list = static_cast<const uint32_t*>(list->ptr); P.n_list = n_list; }
@@ -323,9 +374,10 @@ struct PipelineOp : Op {
     aux.agg = cp->agg;
     fill_table(aux.agg);
     if (deferred_out) {
-      SG_CUDA(cudaMemsetAsync(n_deferred_ptr(), 0, 8, ctx->stream));
+      if (!(next_zeroed && !list)) SG_CUDA(cudaMemsetAsync(n_deferred_ptr(slot), 0, 8, ctx->stream));
+      next_zeroed = false;
       aux.agg.deferred = static_cast<uint32_t*>(deferred_out->ptr);
-      aux.agg.n_deferred = n_deferred_ptr();
+      aux.agg.n_deferred = n_deferred_ptr(slot);
       const char* fl = getenv("SAILGPU_AGG_FIRST_LIMIT");      // tests: force an early hand-back on the first pass
       aux.agg.group_limit = (!list && fl && *fl) ? (unsigned long long)atoll(fl) : ~0ull;   // ~0: launch() derives it from the grid
       // the dictionary variant is only worth running while there are few groups: it hands back early, and the
@@ -395,8 +447,7 @@ struct PipelineOp : Op {
       M.acc_src_word[j] = (int16_t)O.accs[src[(size_t)j]].word;
       M.seen_src[j] = N.accs[j].track_seen ? (O.accs[src[(size_t)j]].track_seen ? (int8_t)src[(size_t)j] : (int8_t)-1) : (int8_t)-2;
     }
-    check_device_error(ctx, run.scal.error());
-    const uint64_t groups = read_n_groups();
+    const uint64_t groups = current_groups();
     AggTable old = tab;
     build_occ(old, O);
     tab.direct = direct_eligible(N);
@@ -415,7 +466,6 @@ struct PipelineOp : Op {
 
   void push_agg(const BatchPtr& b0) {
     Trace tr(ctx, "agg.push");
-    resolve_pending();
     if (b0->rows == 0) return;
     bool widened = false;
     const BatchPtr b = with_union_signature(b0, &widened);
@@ -432,25 +482,50 @@ struct PipelineOp : Op {
     const int64_t tile_rows = (int64_t)cp->rpt * NT;
     const int64_t n_tiles = (b->rows + tile_rows - 1) / tile_rows;
     BufPtr deferred = grouped ? dev_alloc(ctx, (size_t)n_tiles * 4) : nullptr;
-    launch_agg(cp, *b, nullptr, 0, deferred);
+    const int slot = next_slot;
+    launch_agg(cp, *b, nullptr, 0, deferred, slot);
     rows_in_table += b->rows;
     known_groups = -1;
-    if (grouped) { pend.batch = b; pend.cp = cp; pend.deferred = deferred; pend.n_tiles = n_tiles; pend.active = true; }
+    if (!grouped) return;
+    next_slot ^= 1;
+    copy_counters(slot, true);
+    inflight.push_back({b, cp, deferred, slot});
+    settle(1);
   }
 
-  // reads back what the last launch handed back and, until nothing is left, grows the table and re-launches over it
-  void resolve_pending() {
-    if (!pend.active) return;
+  // Looks at the hand-back of every launch in flight but the newest `keep`.  With keep == 0 nothing is left in flight and
+  // known_groups is the table's group count.
+  void settle(size_t keep) {
+    while (inflight.size() > keep) {
+      const InFlight& f = inflight.front();
+      const bool last = inflight.size() == 1;
+      if (last) stream_sync(ctx);          // nothing else queued: this wait drains the stream
+      else SG_CUDA(cudaEventSynchronize(copied[f.slot]));
+      const Counters& c = counters[f.slot];
+      if (c.error || c.n_def[f.slot]) { resolve_all(); return; }
+      if (last) known_groups = (int64_t)c.n_groups;
+      inflight.pop_front();
+    }
+  }
+
+  // Slow path: some launch in flight handed tiles back or raised an error.  Drains the stream, then, until nothing is left,
+  // grows the table for every deferred tile at once and re-launches over each list.
+  void resolve_all() {
     Trace tr(ctx, "agg.resolve");
+    stream_sync(ctx);
+    const Counters* latest = &counters[inflight.back().slot];    // copied after the newest launch: the current values
     uint64_t prev_def = 0;
     for (;;) {
-      unsigned long long gd[3] = {0, 0, 0};      // n_groups @24, cursor @32, n_deferred @40
-      SG_CUDA(cudaMemcpyAsync(gd, run.scal.n_groups(), 24, cudaMemcpyDeviceToHost, ctx->stream));
-      check_device_error(ctx, run.scal.error());   // synchronises
-      const uint64_t groups = gd[0], n_def = gd[2];
-      if (n_def == 0) { known_groups = (int64_t)groups; break; }      // extract_agg() right after needs no second read-back
-      const int64_t tile_rows = (int64_t)pend.cp->rpt * NT;
-      const double rows_def = (double)std::min<int64_t>((int64_t)n_def * tile_rows, pend.batch->rows);
+      raise_device_error(ctx, run.scal.error(), latest->error);
+      const uint64_t groups = latest->n_groups;
+      double rows_def = 0.0;
+      uint64_t n_def_total = 0;
+      for (auto& f : inflight) {
+        const uint64_t n_def = latest->n_def[f.slot];
+        n_def_total += n_def;
+        rows_def += (double)std::min<int64_t>((int64_t)n_def * f.cp->rpt * NT, f.batch->rows);
+      }
+      if (n_def_total == 0) { known_groups = (int64_t)groups; break; }      // extract_agg() right after needs no second read-back
       const double rows_done = std::max(1.0, (double)rows_in_table - rows_def);
       // groups still to come, by the ratio seen so far (every row a new group when nothing was processed yet)
       const double ratio = groups ? std::min(1.0, (double)groups / rows_done) : 1.0;
@@ -458,27 +533,49 @@ struct PipelineOp : Op {
       uint64_t cap = next_pow2((uint64_t)(2.0 * ((double)groups + est)) + 2 * MIN_CAPACITY / 2);
       // a hand-back does not always mean a full table: the dictionary variant gives up at HOT_GROUP_LIMIT groups whatever the
       // capacity.  The table only grows when the estimate asks for it, or when a re-launch at this capacity made no progress.
-      const bool stuck = prev_def != 0 && n_def >= prev_def;
+      const bool stuck = prev_def != 0 && n_def_total >= prev_def;
       if (cap <= tab.capacity && stuck) cap = tab.capacity * 2;
-      prev_def = n_def;
-      if (cap > tab.capacity) alloc_table(pend.cp->agg, cap, groups);
-      std::shared_ptr<CompiledPipeline> cp = pend.cp;
+      prev_def = n_def_total;
+      if (cap > tab.capacity) alloc_table(inflight.front().cp->agg, cap, groups);
       if (!use_cold && groups > CARD_MANY_GROUPS && getenv("SAILGPU_NO_COLD") == nullptr) {
-        auto cold = run.compiled_for(*pend.batch, true);
-        if (cold->agg.entry_words == cp->agg.entry_words) {
-          use_cold = true;                                    // later batches start on the many-groups variant
-          if (cold->rpt == cp->rpt) cp = cold;                // same tile size: this batch's deferred list carries over
-        }
+        auto cold = run.compiled_for(*inflight.front().batch, true);
+        if (cold->agg.entry_words == inflight.front().cp->agg.entry_words) use_cold = true;     // later batches start on the many-groups variant
       }
-      BufPtr next_deferred = dev_alloc(ctx, (size_t)n_def * 4);
-      launch_agg(cp, *pend.batch, pend.deferred, (int64_t)n_def, next_deferred);
-      pend.cp = cp; pend.deferred = next_deferred;
+      for (auto it = inflight.begin(); it != inflight.end();) {
+        const uint64_t n_def = latest->n_def[it->slot];
+        if (n_def == 0) { it = inflight.erase(it); continue; }
+        if (use_cold && !it->cp->cold_variant) {
+          auto cold = run.compiled_for(*it->batch, true);
+          if (cold->rpt == it->cp->rpt && cold->agg.entry_words == it->cp->agg.entry_words) it->cp = cold;   // same tile size: the deferred list carries over
+        }
+        BufPtr next_deferred = dev_alloc(ctx, (size_t)n_def * 4);
+        launch_agg(it->cp, *it->batch, it->deferred, (int64_t)n_def, next_deferred, it->slot);
+        it->deferred = next_deferred;
+        ++it;
+      }
+      const int slot = inflight.back().slot;
+      copy_counters(slot, false);
+      stream_sync(ctx);
+      latest = &counters[slot];
     }
-    pend = Pending();
+    inflight.clear();
+  }
+
+  // the table's group count with nothing in flight (error flag checked)
+  uint64_t current_groups() {
+    settle(0);
+    if (known_groups < 0) {
+      run.ensure_scratch();
+      unsigned long long gd[4] = {0, 0, 0, 0};
+      SG_CUDA(cudaMemcpyAsync(gd, run.scal.buf->ptr, 32, cudaMemcpyDeviceToHost, ctx->stream));      // error flag @0, n_groups @24
+      stream_sync(ctx);
+      raise_device_error(ctx, run.scal.error(), (uint32_t)gd[0]);
+      known_groups = (int64_t)gd[3];
+    }
+    return (uint64_t)known_groups;
   }
 
   BatchPtr extract_agg() {
-    resolve_pending();
     Trace tr(ctx, "agg.extract");
     std::shared_ptr<CompiledPipeline> cp = agg_cp;
     if (!cp) {   // no input at all: compile against an all-valid signature to learn the output layout
@@ -488,11 +585,7 @@ struct PipelineOp : Op {
     }
     const AggParams& A0 = cp->agg;
     run.ensure_scratch();
-    uint64_t groups = 0;
-    if (tab.capacity) {
-      if (known_groups >= 0) groups = (uint64_t)known_groups;
-      else { check_device_error(ctx, run.scal.error()); groups = read_n_groups(); }
-    }
+    const uint64_t groups = tab.capacity ? current_groups() : 0;
     const bool synth = A0.n_keys == 0 && groups == 0;   // global aggregate over zero rows: one row of NULLs / zero counts
     const int64_t rows = synth ? 1 : (int64_t)groups;
     auto out = std::make_shared<DevBatch>();
@@ -534,7 +627,11 @@ struct PipelineOp : Op {
         if (vbytes[(size_t)i] && is_count) SG_CUDA(cudaMemsetAsync(vbytes[(size_t)i]->ptr, 1, 1, ctx->stream));
       }
     }
-    SG_CUDA(cudaMemsetAsync(run.scal.nulls(0), 0, 8 * 20, ctx->stream));
+    // Outputs that cannot be null under this layout (keys without a null word, sums whose inputs carry no validity) have no
+    // validity to pack; only when some output can be null are the null counts read back, so that an all-valid bitmap is dropped
+    bool any_nullable = false;
+    for (int i = 0; i < X.n_cols; ++i) any_nullable |= vbytes[(size_t)i] && rows > 0;
+    if (!any_nullable) return out;
     std::vector<unsigned long long> nulls((size_t)X.n_cols, 0);
     BufPtr nullctr = dev_alloc_zero(ctx, (size_t)X.n_cols * 8 + 8);
     for (int i = 0; i < X.n_cols; ++i) {
@@ -545,7 +642,7 @@ struct PipelineOp : Op {
                                 static_cast<unsigned long long*>(nullctr->ptr) + i, ctx->stream));
     }
     SG_CUDA(cudaMemcpyAsync(nulls.data(), nullctr->ptr, (size_t)X.n_cols * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    SG_CUDA(cudaStreamSynchronize(ctx->stream));
+    stream_sync(ctx);
     for (int i = 0; i < X.n_cols; ++i) {
       DevColumn& c = out->cols[(size_t)i];
       if (c.validity) { c.null_count = (int64_t)nulls[(size_t)i]; if (c.null_count == 0) c.validity = nullptr; }
@@ -639,13 +736,26 @@ std::unique_ptr<Op> make_op(Ctx* ctx, const Json& spec, const std::vector<Schema
     SG_CHECK(op->run.stages[i].kind != StageSpec::Aggregate, SAILGPU_ERR_INVALID, "aggregate must be the last stage of a pipeline");
   op->out_schema = cur;
   // a group key the hash table cannot pack (more than 6 keys / 64 bytes): grouping by sorting instead (ops_more.cu WideAggOp)
+  // The verdict depends on the spec and the input schema only: it is kept with the operator's compiled pipelines, so that
+  // re-creating the same plan (every execution of a query) compiles nothing on the host.
   if (kind == "aggregate" && !g_in_static_check) {
-    bool wide = false;
-    g_in_static_check = true;
-    try { pipeline_static_check(spec, inputs); }
-    catch (const Error& e) { wide = e.code == SAILGPU_ERR_UNSUPPORTED && std::string(e.what()).find("group key") != std::string::npos; }
-    g_in_static_check = false;
-    if (wide) return make_wide_agg_op(ctx, spec, inputs, cur);
+    std::shared_ptr<bool> verdict;
+    const std::string vkey = "wide_agg|" + op->share_key;
+    const bool cacheable = ctx && ctx->stream != nullptr;
+    if (cacheable) {
+      auto it = ctx->shared_objects.find(vkey);
+      if (it != ctx->shared_objects.end()) verdict = std::static_pointer_cast<bool>(it->second);
+    }
+    if (!verdict) {
+      bool wide = false;
+      g_in_static_check = true;
+      try { pipeline_static_check(spec, inputs); }
+      catch (const Error& e) { wide = e.code == SAILGPU_ERR_UNSUPPORTED && std::string(e.what()).find("group key") != std::string::npos; }
+      g_in_static_check = false;
+      verdict = std::make_shared<bool>(wide);
+      if (cacheable) ctx->shared_objects.emplace(vkey, std::static_pointer_cast<void>(verdict));
+    }
+    if (*verdict) return make_wide_agg_op(ctx, spec, inputs, cur);
   }
   return op;
 }

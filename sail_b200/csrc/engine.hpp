@@ -16,6 +16,7 @@ struct Metrics {
   uint64_t elapsed_compute_ns = 0, kernel_launches = 0;
   uint64_t build_input_rows = 0, build_input_batches = 0, build_time_ns = 0, join_time_ns = 0;
   uint64_t pipeline_launches = 0, pipeline_kernel_ns = 0, jit_launches = 0;
+  uint64_t host_syncs = 0;      // stream drains during calls on this operator's handle (import and export included), capi.cu
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> pending;   // CUDA events bracketing each pipeline-kernel launch
 };
 

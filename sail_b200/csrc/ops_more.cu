@@ -397,7 +397,7 @@ struct JoinOp : Op {
     const int64_t nblocks = std::min<int64_t>(1024, (n + 4095) / 4096);
     uint64_t total = 0;
     SG_CUDA(cudaMemcpyAsync(&total, static_cast<uint64_t*>(scratch->ptr) + nblocks, 8, cudaMemcpyDeviceToHost, ctx->stream));
-    SG_CUDA(cudaStreamSynchronize(ctx->stream));
+    stream_sync(ctx);
     if (total == 0) return;
     BufPtr ob = dev_alloc(ctx, (size_t)total * 8), op = dev_alloc(ctx, (size_t)total * 8);
     J.offsets = static_cast<const uint64_t*>(offs->ptr); J.out_build = static_cast<int64_t*>(ob->ptr); J.out_probe = static_cast<int64_t*>(op->ptr);
@@ -409,7 +409,7 @@ struct JoinOp : Op {
     out->rows = (int64_t)total;
     for (size_t i = 0; i < bs.size(); ++i) out->cols.push_back(gather_column(build->cols[i], bs[i], J.out_build, (int64_t)total, jt == "right"));
     for (size_t i = 0; i < ps.size(); ++i) out->cols.push_back(gather_column(b->cols[i], ps[i], J.out_probe, (int64_t)total, false));
-    SG_CUDA(cudaStreamSynchronize(ctx->stream));
+    stream_sync(ctx);
     ready.push_back(post_filter(out));
   }
 
@@ -724,20 +724,20 @@ struct NestedLoopJoinOp : Op {
     if (c.validity) {
       uint8_t byte = 0;
       SG_CUDA(cudaMemcpyAsync(&byte, static_cast<const uint8_t*>(c.validity->ptr) + (row >> 3), 1, cudaMemcpyDeviceToHost, ctx->stream));
-      SG_CUDA(cudaStreamSynchronize(ctx->stream));
+      stream_sync(ctx);
       if (!((byte >> (row & 7)) & 1)) { e->lit_null = true; e->nullable = true; return e; }
     }
     if (t.id == TypeId::Bool) {
       uint8_t byte = 0;
       SG_CUDA(cudaMemcpyAsync(&byte, static_cast<const uint8_t*>(c.data->ptr) + (row >> 3), 1, cudaMemcpyDeviceToHost, ctx->stream));
-      SG_CUDA(cudaStreamSynchronize(ctx->stream));
+      stream_sync(ctx);
       e->lit_i = (byte >> (row & 7)) & 1;
       return e;
     }
     const int w = t.is_string() ? 16 : t.arrow_width();
     uint8_t raw[16] = {0};
     SG_CUDA(cudaMemcpyAsync(raw, static_cast<const uint8_t*>(c.data->ptr) + row * w, (size_t)w, cudaMemcpyDeviceToHost, ctx->stream));
-    SG_CUDA(cudaStreamSynchronize(ctx->stream));
+    stream_sync(ctx);
     if (t.is_string()) {
       uint32_t len; memcpy(&len, raw, 4);
       e->lit_s.resize(len);
@@ -745,7 +745,7 @@ struct NestedLoopJoinOp : Op {
       else {
         uint64_t ptr; memcpy(&ptr, raw + 8, 8);       // resolved view: absolute device pointer
         SG_CUDA(cudaMemcpyAsync(&e->lit_s[0], reinterpret_cast<const void*>(ptr), len, cudaMemcpyDeviceToHost, ctx->stream));
-        SG_CUDA(cudaStreamSynchronize(ctx->stream));
+        stream_sync(ctx);
       }
     } else if (t.id == TypeId::Float64) { memcpy(&e->lit_f, raw, 8); }
     else if (t.id == TypeId::Float32) { float f; memcpy(&f, raw, 4); e->lit_f = f; }
@@ -878,14 +878,11 @@ struct SortOp : Op {
 
   struct Encoded { BufPtr keys, bits; int key_bytes = 0; };
 
-  // order-preserving fixed-width encoding of the sort keys of every row (memcmp order == requested order)
-  Encoded encode_keys(const BatchPtr& all, const Schema& sch, const std::vector<Key>& ks) {
-    const int64_t n = all->rows;
+  // the key columns of every row as the encoder and the small sort read them (string keys: no length bound yet)
+  SortEncodeParams describe_keys(const BatchPtr& all, const Schema& sch, const std::vector<Key>& ks) {
     SortEncodeParams E; memset(&E, 0, sizeof(E));
-    E.n = n; E.n_keys = (int)ks.size();
-    int off = 0;
-    BufPtr maxlen = dev_alloc_zero(ctx, 8 * 8);
-    std::vector<int> str_keys;
+    E.n = all->rows; E.n_keys = (int)ks.size();
+    SG_CHECK(ks.size() <= sizeof(E.cols) / sizeof(E.cols[0]), SAILGPU_ERR_UNSUPPORTED, "more than 8 sort keys");
     for (size_t k = 0; k < ks.size(); ++k) {
       SG_CHECK(ks[k].e->kind == Expr::Col, SAILGPU_ERR_UNSUPPORTED, "sort keys must be column references");
       const DevColumn& c = all->cols[(size_t)ks[k].e->col];
@@ -894,16 +891,28 @@ struct SortOp : Op {
       s.data = static_cast<const uint8_t*>(c.data->ptr);
       s.validity_bits = c.validity ? static_cast<const uint8_t*>(c.validity->ptr) : nullptr;
       s.asc = ks[k].asc; s.nulls_first = ks[k].nulls_first;
-      if (t.is_string()) { s.kind = SORT_VIEW; s.width = 16; SG_CUDA(launch_max_view_len(c.data->ptr, n, static_cast<unsigned int*>(maxlen->ptr) + k, ctx->stream)); str_keys.push_back((int)k); }
+      if (t.is_string()) { s.kind = SORT_VIEW; s.width = 16; }
       else if (t.id == TypeId::Bool) { s.kind = SORT_BOOL; s.width = 1; s.enc_bytes = 1; }
       else if (t.is_float()) { SG_CHECK(t.id == TypeId::Float64, SAILGPU_ERR_UNSUPPORTED, "Float32 sort keys"); s.kind = SORT_F64; s.width = 8; s.enc_bytes = 8; }
       else if (t.is_unsigned_int()) { s.kind = SORT_UINT; s.width = t.arrow_width(); s.enc_bytes = s.width; }
       else { s.kind = SORT_INT; s.width = t.arrow_width(); s.enc_bytes = s.width; }
     }
+    return E;
+  }
+
+  // order-preserving fixed-width encoding of the sort keys of every row (memcmp order == requested order)
+  Encoded encode_keys(const BatchPtr& all, const Schema& sch, const std::vector<Key>& ks) {
+    const int64_t n = all->rows;
+    SortEncodeParams E = describe_keys(all, sch, ks);
+    int off = 0;
+    BufPtr maxlen = dev_alloc_zero(ctx, 8 * 8);
+    std::vector<int> str_keys;
+    for (size_t k = 0; k < ks.size(); ++k)
+      if (E.cols[k].kind == SORT_VIEW) { SG_CUDA(launch_max_view_len(E.cols[k].data, n, static_cast<unsigned int*>(maxlen->ptr) + k, ctx->stream)); str_keys.push_back((int)k); }
     if (!str_keys.empty()) {
       unsigned int lens[8] = {0};
       SG_CUDA(cudaMemcpyAsync(lens, maxlen->ptr, sizeof(lens), cudaMemcpyDeviceToHost, ctx->stream));
-      SG_CUDA(cudaStreamSynchronize(ctx->stream));
+      stream_sync(ctx);
       for (int k : str_keys) {
         SG_CHECK(lens[k] <= 256, SAILGPU_ERR_UNSUPPORTED, "sort key strings longer than 256 bytes are not supported yet");
         E.cols[k].str_len = (int)lens[k]; E.cols[k].enc_bytes = (int)lens[k] + 4;
@@ -931,11 +940,22 @@ struct SortOp : Op {
     return out;
   }
 
-  // full sort: LSD radix over the encoded keys (stable), then one gather per column
+  // full sort: LSD radix over the encoded keys (stable), then one gather per column.  Up to SMALL_SORT_ROWS rows are ranked
+  // by one CTA straight from the key columns, without an encoding and without reading anything back.  Nothing here waits for
+  // the device: every temporary is released in stream order (device.hpp, size-class cache).
   BatchPtr sort_rows(const BatchPtr& all, const Schema& sch, const std::vector<Key>& ks, int64_t limit) {
     const int64_t n = all->rows;
     if (n == 0) return all;
     SG_CHECK(n < (1ll << 32), SAILGPU_ERR_UNSUPPORTED, "sort of more than 2^32 rows in one partition");
+    const int64_t take = limit >= 0 ? std::min<int64_t>(limit, n) : n;
+    if (n <= SMALL_SORT_ROWS) {
+      const SortEncodeParams E = describe_keys(all, sch, ks);
+      BufPtr order = dev_alloc(ctx, (size_t)n * 4), idx = dev_alloc(ctx, (size_t)take * 8);
+      SG_CUDA(launch_small_sort_cols(E, static_cast<uint32_t*>(order->ptr), ctx->stream));
+      SG_CUDA(launch_widen_u32(static_cast<const uint32_t*>(order->ptr), static_cast<int64_t*>(idx->ptr), take, ctx->stream));
+      m.kernel_launches += 2;
+      return take_rows(all, sch, static_cast<const int64_t*>(idx->ptr), take);
+    }
     Encoded enc = encode_keys(all, sch, ks);
     const int64_t n_chunks = (n + 2047) / 2048;
     BufPtr ia = dev_alloc(ctx, (size_t)n * 4), ib = dev_alloc(ctx, (size_t)n * 4), ka = dev_alloc(ctx, (size_t)n * 8), kbuf = dev_alloc(ctx, (size_t)n * 8),
@@ -947,12 +967,9 @@ struct SortOp : Op {
     int sort_launches = 0;
     SG_CUDA(radix_sort_indices(static_cast<const uint8_t*>(enc.keys->ptr), enc.key_bytes, n, S, static_cast<const uint32_t*>(enc.bits->ptr), ctx->stream, &sort_launches));
     m.kernel_launches += (uint64_t)(sort_launches + 1);
-    const int64_t take = limit >= 0 ? std::min<int64_t>(limit, n) : n;
     BufPtr idx = dev_alloc(ctx, (size_t)take * 8);
     SG_CUDA(launch_widen_u32(static_cast<const uint32_t*>(ia->ptr), static_cast<int64_t*>(idx->ptr), take, ctx->stream));
-    BatchPtr out = take_rows(all, sch, static_cast<const int64_t*>(idx->ptr), take);
-    SG_CUDA(cudaStreamSynchronize(ctx->stream));
-    return out;
+    return take_rows(all, sch, static_cast<const int64_t*>(idx->ptr), take);
   }
 
   // TopK: radix-select the rows that can be among the first `k` on the leading 8 key bytes (one 8 B/row pass per 11 bits),
@@ -975,7 +992,7 @@ struct SortOp : Op {
       SG_CUDA(cudaMemsetAsync(hist->ptr, 0, 2048 * 4, ctx->stream));
       SG_CUDA(launch_topk_hist(kp, enc.key_bytes, n, used, prefix, db, static_cast<uint32_t*>(hist->ptr), ctx->stream));
       SG_CUDA(cudaMemcpyAsync(h.data(), hist->ptr, 2048 * 4, cudaMemcpyDeviceToHost, ctx->stream));
-      SG_CUDA(cudaStreamSynchronize(ctx->stream));
+      stream_sync(ctx);
       m.kernel_launches += 1;
       int64_t run = below;
       int bin = 0;
@@ -1070,7 +1087,7 @@ struct MergeOp : SortOp {
           BufPtr idx = dev_alloc(ctx, (size_t)fetch * 8);
           SG_CUDA(launch_iota(static_cast<int64_t*>(idx->ptr), fetch, ctx->stream));
           r = take_rows(r, sch, static_cast<const int64_t*>(idx->ptr), fetch);
-          SG_CUDA(cudaStreamSynchronize(ctx->stream));
+          stream_sync(ctx);
         }
     if (runs.size() == 1) return runs[0];
     std::vector<int64_t> off(runs.size() + 1, 0);
@@ -1085,7 +1102,7 @@ struct MergeOp : SortOp {
     m.kernel_launches += 1;
     const int64_t take = fetch >= 0 ? std::min<int64_t>(fetch, n) : n;
     BatchPtr out = take_rows(all, sch, static_cast<const int64_t*>(perm->ptr), take);
-    SG_CUDA(cudaStreamSynchronize(ctx->stream));       // `off` is a host vector
+    stream_sync(ctx);       // `off` is a host vector
     return out;
   }
 };
@@ -1221,7 +1238,7 @@ struct WideAggOp : Op {
                                static_cast<const uint8_t*>(hk->ptr), static_cast<unsigned long long*>(coll->ptr), ctx->stream));
     unsigned long long n_coll = 0;
     SG_CUDA(cudaMemcpyAsync(&n_coll, coll->ptr, 8, cudaMemcpyDeviceToHost, ctx->stream));
-    SG_CUDA(cudaStreamSynchronize(ctx->stream));
+    stream_sync(ctx);
     if (n_coll != 0 || getenv("SAILGPU_WIDEAGG_FULL_SORT") != nullptr) {
       int more = 0;
       SG_CUDA(radix_sort_indices(static_cast<const uint8_t*>(enc.keys->ptr), enc.key_bytes, n, S, static_cast<const uint32_t*>(enc.bits->ptr), ctx->stream, &more));
@@ -1231,7 +1248,7 @@ struct WideAggOp : Op {
     SG_CUDA(launch_exclusive_scan_u32(static_cast<const uint32_t*>(heads->ptr), n, static_cast<uint64_t*>(before->ptr), static_cast<uint64_t*>(scr2->ptr), ctx->stream));
     uint64_t n_groups = 0;
     SG_CUDA(cudaMemcpyAsync(&n_groups, static_cast<uint64_t*>(scr2->ptr) + std::min<int64_t>(1024, (n + 4095) / 4096), 8, cudaMemcpyDeviceToHost, ctx->stream));
-    SG_CUDA(cudaStreamSynchronize(ctx->stream));
+    stream_sync(ctx);
     DevColumn gid; gid.type = T(TypeId::Int64); gid.length = n; gid.data = dev_alloc(ctx, (size_t)n * 8);
     BufPtr rep = dev_alloc(ctx, (size_t)n_groups * 8);
     SG_CUDA(launch_assign_groups(S.idx_a, static_cast<const uint32_t*>(heads->ptr), static_cast<const uint64_t*>(before->ptr), n,
@@ -1272,7 +1289,7 @@ struct WideAggOp : Op {
     }
     for (size_t i = 1; i < agg->cols.size(); ++i) out->cols.push_back(agg->cols[i]);
     m.kernel_launches += (uint64_t)n_keys + 1;
-    SG_CUDA(cudaStreamSynchronize(ctx->stream));
+    stream_sync(ctx);
     return out;
   }
 };
@@ -1322,7 +1339,7 @@ struct RepartitionOp : Op {
       ready[(size_t)p].push_back(pb);
     }
     next_idx = (next_idx + n) % n_parts;
-    SG_CUDA(cudaStreamSynchronize(ctx->stream));       // the index vectors are released on return
+    stream_sync(ctx);       // the index vectors are released on return
   }
 
   void push(int input, const BatchPtr& b) override {
@@ -1371,7 +1388,7 @@ struct RepartitionOp : Op {
     run.launch(P, cp, &aux, m);
     std::vector<int64_t> cnt((size_t)n_parts), off((size_t)n_parts);
     SG_CUDA(cudaMemcpyAsync(cnt.data(), counts->ptr, (size_t)n_parts * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    SG_CUDA(cudaStreamSynchronize(ctx->stream));
+    stream_sync(ctx);
     int64_t run_off = 0;
     for (int p = 0; p < n_parts; ++p) { off[(size_t)p] = run_off; run_off += cnt[(size_t)p]; }
     SG_CUDA(cudaMemcpyAsync(offsets->ptr, off.data(), (size_t)n_parts * 8, cudaMemcpyHostToDevice, ctx->stream));
@@ -1425,7 +1442,7 @@ struct RepartitionOp : Op {
       }
       ready[(size_t)p].push_back(pb);
     }
-    SG_CUDA(cudaStreamSynchronize(ctx->stream));
+    stream_sync(ctx);
   }
 };
 
@@ -1500,7 +1517,7 @@ struct ExchangeOp : Op {
       auto b = std::make_shared<DevBatch>();
       b->rows = k;
       for (size_t c = 0; c < sch.size(); ++c) b->cols.push_back(helper.gather_column(result->cols[c], sch[c], static_cast<const int64_t*>(idx->ptr), k, false));
-      SG_CUDA(cudaStreamSynchronize(ctx->stream));
+      stream_sync(ctx);
       run_batches.push_back(b);
     }
     if (run_batches.empty()) run_batches.push_back(result);
@@ -1745,7 +1762,7 @@ BatchPtr exchange_batches(Ctx* ctx, const Schema& schema, const std::vector<Batc
   NCCL_CALL(g_nccl.AllGather(dmine->ptr, dall->ptr, mine.size(), NCCL_INT64, ctx->nccl_comm, ctx->stream));
   std::vector<int64_t> all(mine.size() * (size_t)W);
   SG_CUDA(cudaMemcpyAsync(all.data(), dall->ptr, all.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
-  SG_CUDA(cudaStreamSynchronize(ctx->stream));                                                                  // the one synchronisation
+  stream_sync(ctx);                                                                  // the one synchronisation
   auto cnt = [&](int src, int dst, size_t field) { return all[((size_t)src * W + dst) * rec + field]; };
   if (abort_above_rows >= 0) {
     int64_t mx = 0;

@@ -401,7 +401,7 @@ DevColumn decode_parquet_column(Ctx* ctx, const Field& f, const ParquetColumnDes
     expand_runs_kernel<<<(int)std::min<int64_t>((n + 255) / 256, grid_cap(8)), 256, 0, ctx->stream>>>(dbase, static_cast<const Run*>(druns->ptr), static_cast<const int64_t*>(dstarts->ptr),
                                                                                                 (int)runs.size(), n, static_cast<uint32_t*>(out->ptr));
     SG_CUDA(cudaGetLastError());
-    SG_CUDA(cudaStreamSynchronize(ctx->stream));      // `starts` / `runs` are host vectors
+    stream_sync(ctx);      // `starts` / `runs` are host vectors
     return out;
   };
   DecodeParams D; memset(&D, 0, sizeof(D));
@@ -438,7 +438,7 @@ DevColumn decode_parquet_column(Ctx* ctx, const Field& f, const ParquetColumnDes
     ddict = dev_alloc(ctx, (size_t)std::max<int64_t>(dict_count, 1) * out_width);
     if (dict_count) decode_values_kernel<<<(int)std::min<int64_t>((dict_count + 255) / 256, grid_cap(4)), 256, 0, ctx->stream>>>(Q, static_cast<uint8_t*>(ddict->ptr));
     SG_CUDA(cudaGetLastError());
-    SG_CUDA(cudaStreamSynchronize(ctx->stream));
+    stream_sync(ctx);
     didx = expand(index_runs, dense_done);
     D.dict_idx = static_cast<const uint32_t*>(didx->ptr); D.dict_vals = static_cast<const uint8_t*>(ddict->ptr); D.dict_size = (uint32_t)dict_count;
   }
@@ -465,7 +465,7 @@ DevColumn decode_parquet_column(Ctx* ctx, const Field& f, const ParquetColumnDes
   }
   uint32_t e = 0;
   SG_CUDA(cudaMemcpyAsync(&e, err->ptr, 4, cudaMemcpyDeviceToHost, ctx->stream));
-  SG_CUDA(cudaStreamSynchronize(ctx->stream));       // host vectors above; error flag
+  stream_sync(ctx);       // host vectors above; error flag
   SG_CHECK(e == 0, SAILGPU_ERR_INVALID, "parquet: dictionary index out of range in column '" + f.name + "'");
   return col;
 }

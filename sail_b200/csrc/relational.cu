@@ -298,6 +298,67 @@ __global__ void small_sort_kernel(const uint8_t* __restrict__ keys, int key_byte
   idx_out[rank] = (uint32_t)i;
 }
 
+// n <= 1024 without an encoding pass: one CTA ranks every row against every other by comparing the key columns in place,
+// in exactly the order sort_encode_kernel's bytes give (stable: ties broken by input position).  Strings are compared as
+// they are, so no bound on their length has to be known beforehand.
+__device__ int cmp_sort_key(const SortKeyCol& c, int64_t a, int64_t b) {
+  const bool na = c.validity_bits && !((c.validity_bits[a >> 3] >> (a & 7)) & 1);
+  const bool nb = c.validity_bits && !((c.validity_bits[b >> 3] >> (b & 7)) & 1);
+  if (na || nb) return na == nb ? 0 : ((na == (c.nulls_first != 0)) ? -1 : 1);
+  int r = 0;
+  switch (c.kind) {
+    case SORT_INT:
+    case SORT_UINT: {        // most significant byte first, sign bit flipped for signed integers
+      const uint8_t* pa = c.data + a * c.width;
+      const uint8_t* pb = c.data + b * c.width;
+      for (int i = 0; i < c.width && r == 0; ++i) {
+        const uint8_t f = (i == 0 && c.kind == SORT_INT) ? 0x80 : 0x00;
+        r = (int)(pa[c.width - 1 - i] ^ f) - (int)(pb[c.width - 1 - i] ^ f);
+      }
+      break;
+    }
+    case SORT_F64: {
+      uint64_t x = *reinterpret_cast<const uint64_t*>(c.data + a * 8), y = *reinterpret_cast<const uint64_t*>(c.data + b * 8);
+      x = (x >> 63) ? ~x : (x | 0x8000000000000000ull);
+      y = (y >> 63) ? ~y : (y | 0x8000000000000000ull);
+      r = x < y ? -1 : (x > y ? 1 : 0);
+      break;
+    }
+    case SORT_BOOL:
+      r = (int)((c.data[a >> 3] >> (a & 7)) & 1) - (int)((c.data[b >> 3] >> (b & 7)) & 1);
+      break;
+    default: {               // SORT_VIEW: bytes, the shorter string padded with zeros, then the length
+      const uint8_t* va = c.data + a * 16;
+      const uint8_t* vb = c.data + b * 16;
+      const ulonglong2 x = *reinterpret_cast<const ulonglong2*>(va), y = *reinterpret_cast<const ulonglong2*>(vb);
+      const uint32_t la = (uint32_t)x.x, lb = (uint32_t)y.x;
+      const uint8_t* sa = view_ptr(x, va);
+      const uint8_t* sb = view_ptr(y, vb);
+      const uint32_t m = la > lb ? la : lb;
+      for (uint32_t i = 0; i < m && r == 0; ++i) r = (int)(i < la ? sa[i] : 0) - (int)(i < lb ? sb[i] : 0);
+      if (r == 0) r = la < lb ? -1 : (la > lb ? 1 : 0);
+    }
+  }
+  return c.asc ? r : -r;
+}
+__global__ void small_sort_cols_kernel(const SortEncodeParams P, uint32_t* __restrict__ idx_out) {
+  const int i = threadIdx.x;
+  if (i >= P.n) return;
+  int rank = 0;
+  for (int j = 0; j < (int)P.n; ++j) {
+    int c = 0;
+    for (int k = 0; k < P.n_keys && c == 0; ++k) c = cmp_sort_key(P.cols[k], j, i);
+    rank += (c < 0 || (c == 0 && j < i)) ? 1 : 0;
+  }
+  idx_out[rank] = (uint32_t)i;
+}
+cudaError_t launch_small_sort_cols(const SortEncodeParams& P, uint32_t* idx_out, cudaStream_t s) {
+  if (P.n == 0) return cudaSuccess;
+  if (P.n > SMALL_SORT_ROWS) return cudaErrorInvalidValue;
+  small_sort_cols_kernel<<<1, SMALL_SORT_ROWS, 0, s>>>(P, idx_out);
+  return cudaGetLastError();
+}
+
 // Sorts row indices by the encoded keys; `S.idx_a` receives the final order.  `bits` = the [2 * key_bytes] words
 // sort_encode_kernel filled.  Synchronises the stream once (to read `bits`).  *launches counts the kernels issued.
 cudaError_t radix_sort_indices(const uint8_t* keys, int key_bytes, int64_t n, const RadixScratch& S, const uint32_t* bits, cudaStream_t s, int* launches) {

@@ -64,6 +64,9 @@ cudaError_t launch_join_multi(const JoinMultiParams& P, cudaStream_t s);
 cudaError_t launch_gather_bits(const uint8_t* bits, uint8_t* out, const int64_t* idx, int64_t n, int dflt, cudaStream_t s);
 cudaError_t launch_max_view_len(const void* views, int64_t n, unsigned int* out, cudaStream_t s);
 cudaError_t launch_sort_encode(const SortEncodeParams& P, cudaStream_t s);
+// P.n <= SMALL_SORT_ROWS rows ordered by the key columns of P (no `keys` / `bits` needed): idx_out[rank] = row
+constexpr int SMALL_SORT_ROWS = 1024;
+cudaError_t launch_small_sort_cols(const SortEncodeParams& P, uint32_t* idx_out, cudaStream_t s);
 cudaError_t radix_sort_indices(const uint8_t* keys, int key_bytes, int64_t n, const RadixScratch& S, const uint32_t* bits, cudaStream_t s, int* launches);
 cudaError_t launch_topk_hist(const uint8_t* keys, int key_bytes, int64_t n, int used, uint64_t prefix, int digit_bits, uint32_t* hist /* [2048], zeroed */, cudaStream_t s);
 cudaError_t launch_topk_compact(const uint8_t* keys, int key_bytes, int64_t n, int used, uint64_t threshold, int64_t* out, unsigned long long* counter, cudaStream_t s);

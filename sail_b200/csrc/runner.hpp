@@ -129,7 +129,7 @@ struct PipelineRunner {
       }
       if (!cp->literals.empty()) {
         SG_CUDA(cudaMemcpyAsync(dp.literals->ptr, blob.data(), blob.size(), cudaMemcpyHostToDevice, ctx->stream));
-        SG_CUDA(cudaStreamSynchronize(ctx->stream));   // host blob goes out of scope
+        stream_sync(ctx);   // host blob goes out of scope
       }
       for (auto& fx : cp->literal_fixups) cp->prog[(size_t)fx.first].imm1 = dp.literal_ptrs[(size_t)fx.second];
       it = programs.emplace(cp.get(), std::move(dp)).first;
@@ -317,7 +317,7 @@ inline BatchPtr run_streaming(PipelineRunner& run, Ctx* ctx, const BatchPtr& b, 
         c.null_count = -1;
       }
     }
-    if (!bool_tmp.empty() || !valid_tmp.empty()) SG_CUDA(cudaStreamSynchronize(ctx->stream));
+    if (!bool_tmp.empty() || !valid_tmp.empty()) stream_sync(ctx);
   } else {
     check_device_error(ctx, run.scal.error());
   }
