@@ -190,22 +190,32 @@ SAILGPU_API int32_t sailgpu_spec_validate(const char* spec_json, size_t spec_len
  * decoded on the device (page headers and RLE run headers are walked on the host, every value is produced by a GPU thread).
  * `schema` names the Arrow type each column decodes to (Int32/Date32, Int64, Float64, Decimal128 from FIXED_LEN_BYTE_ARRAY /
  * INT32 / INT64, Utf8View from BYTE_ARRAY).  Covered: data pages V1/V2, PLAIN and dictionary encodings, flat optional columns,
- * uncompressed pages; anything else returns SAILGPU_ERR_UNSUPPORTED and the caller keeps its CPU reader for that file. */
+ * uncompressed and ZSTD-compressed pages (codec 0 or 6; columns of both kinds may be mixed in one call); anything else, and
+ * ZSTD frames that need a dictionary, returns SAILGPU_ERR_UNSUPPORTED and the caller keeps its CPU reader for that file.
+ * ZSTD pages are decompressed on the device by one launch per call, covering every column; the decompressed chunk is read
+ * back to the host once, because the RLE run headers are walked there.  A corrupt ZSTD page returns SAILGPU_ERR_INVALID
+ * with a message naming the column and the page. */
 typedef struct sailgpu_parquet_column {
   const uint8_t* chunk;      /* host pointer: first byte of the column chunk (its dictionary page, else its first data page) */
   uint64_t chunk_len;        /* total_compressed_size of the chunk */
   int32_t physical_type;     /* parquet::Type: 1 INT32, 2 INT64, 5 DOUBLE, 6 BYTE_ARRAY, 7 FIXED_LEN_BYTE_ARRAY */
   int32_t type_length;       /* FIXED_LEN_BYTE_ARRAY length, else 0 */
   int32_t max_def_level;     /* 0 required, 1 optional */
-  int32_t codec;             /* parquet::CompressionCodec: 0 UNCOMPRESSED */
+  int32_t codec;             /* parquet::CompressionCodec: 0 UNCOMPRESSED, 6 ZSTD */
   int64_t num_values;
 } sailgpu_parquet_column;
 SAILGPU_API int32_t sailgpu_parquet_decode(sailgpu_ctx* ctx, const struct ArrowSchema* schema, const sailgpu_parquet_column* cols,
                                            int32_t n_cols, int64_t n_rows, struct ArrowDeviceArray* out);
 /* Plan-time / diagnostic companion: walks the pages and run headers of column `column` on the host only and reports what it
- * found as JSON ({"pages":..,"dense":non-null values,"dict_count":..,...}); fails exactly where sailgpu_parquet_decode would. */
+ * found as JSON ({"pages":..,"dense":non-null values,"dict_count":..,...,"body_bytes":..,"body_fnv1a":..}); fails exactly where
+ * sailgpu_parquet_decode would.  body_bytes / body_fnv1a: length and FNV-1a 64 hash of the page bodies walked, in page order,
+ * after decompression (a ZSTD chunk is decompressed on the host by the decoder the device runs). */
 SAILGPU_API int32_t sailgpu_parquet_inspect(const struct ArrowSchema* schema, const sailgpu_parquet_column* cols, int32_t n_cols,
                                             int64_t n_rows, int32_t column, char* buf, size_t cap);
+/* What the last sailgpu_parquet_decode call on `ctx` spent on ZSTD pages, as JSON: {"zstd_pages":..,"zstd_out_bytes":..,
+ * "image_bytes":..,"decompress_ms":..,"readback_ms":..} (device time of the decompression launch and of the image read-back,
+ * from CUDA events; all zero when the call had no ZSTD column). */
+SAILGPU_API int32_t sailgpu_parquet_stats(sailgpu_ctx* ctx, char* buf, size_t cap);
 
 /* Plan-time kernel specialisation.  The library interprets any pipeline at once and, for pipelines that see enough
  * rows (SAILGPU_JIT_MIN_ROWS, default 4 Mi), compiles a specialised sm_90a kernel with NVRTC the first time; the

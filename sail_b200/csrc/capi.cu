@@ -52,7 +52,7 @@ size_t pipeline_precompile(const Json& spec, const std::vector<Schema>& inputs, 
 
 namespace sg {
 struct ParquetColumnDesc { const uint8_t* chunk; uint64_t chunk_len; int32_t physical_type, type_length, max_def_level, codec; int64_t num_values; };
-DevColumn decode_parquet_column(Ctx* ctx, const Field& f, const ParquetColumnDesc& c, int64_t n_rows);
+void decode_parquet_row_group(Ctx* ctx, const Schema& schema, const std::vector<ParquetColumnDesc>& cols, int64_t n_rows, DevBatch* b);
 std::string parquet_plan_summary(const Field& f, const ParquetColumnDesc& c, int64_t n_rows);
 }
 
@@ -196,11 +196,20 @@ SAILGPU_API int32_t sailgpu_parquet_decode(sailgpu_ctx* c, const struct ArrowSch
     SG_CHECK((int)schema.size() == n_cols, SAILGPU_ERR_INVALID, "parquet: " + std::to_string(n_cols) + " column chunks for a schema of " + std::to_string(schema.size()) + " fields");
     auto b = std::make_shared<DevBatch>();
     b->rows = n_rows;
-    for (int i = 0; i < n_cols; ++i) {
-      ParquetColumnDesc d{cols[i].chunk, cols[i].chunk_len, cols[i].physical_type, cols[i].type_length, cols[i].max_def_level, cols[i].codec, cols[i].num_values};
-      b->cols.push_back(decode_parquet_column(&c->ctx, schema[(size_t)i], d, n_rows));
-    }
+    std::vector<ParquetColumnDesc> descs;
+    for (int i = 0; i < n_cols; ++i)
+      descs.push_back(ParquetColumnDesc{cols[i].chunk, cols[i].chunk_len, cols[i].physical_type, cols[i].type_length, cols[i].max_def_level, cols[i].codec, cols[i].num_values});
+    decode_parquet_row_group(&c->ctx, schema, descs, n_rows, b.get());
     export_device_batch(&c->ctx, schema, b, out);
+  });
+}
+SAILGPU_API int32_t sailgpu_parquet_stats(sailgpu_ctx* c, char* buf, size_t cap) {
+  return guard(&g_ctx_error, [&] {
+    SG_CHECK(c && buf && cap, SAILGPU_ERR_INVALID, "null argument");
+    CtxLock lk(c->ctx.mu);
+    const Ctx::ParquetZstd& s = c->ctx.parquet_zstd;
+    snprintf(buf, cap, "{\"zstd_pages\":%llu,\"zstd_out_bytes\":%llu,\"image_bytes\":%llu,\"decompress_ms\":%.4f,\"readback_ms\":%.4f}", (unsigned long long)s.pages,
+             (unsigned long long)s.out_bytes, (unsigned long long)s.image_bytes, (double)s.decompress_ms, (double)s.readback_ms);
   });
 }
 

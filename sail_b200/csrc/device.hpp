@@ -71,6 +71,10 @@ struct Ctx {
   void* pinned_block = nullptr;
   std::vector<uint32_t> pinned_free;
   uint32_t pinned_next = 0;
+  // the ZSTD work of the last sailgpu_parquet_decode call (parquet.cu; sailgpu_parquet_stats): pages, bytes they decompressed
+  // to, bytes read back, and the device time of the decompression launch and of the read-back (CUDA events)
+  struct ParquetZstd { uint64_t pages = 0, out_bytes = 0, image_bytes = 0; float decompress_ms = 0, readback_ms = 0; };
+  ParquetZstd parquet_zstd;
 };
 
 // Waits until everything queued on the context's stream has run.  Every such wait leaves the device without work until the

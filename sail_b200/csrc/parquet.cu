@@ -9,13 +9,22 @@
 //
 // Covered: data pages V1 / V2, dictionary pages, PLAIN and RLE_DICTIONARY / PLAIN_DICTIONARY values, RLE definition
 // levels of flat optional columns (max level 1), physical types INT32 / INT64 / DOUBLE / FLOAT / FIXED_LEN_BYTE_ARRAY /
-// BYTE_ARRAY, uncompressed pages.  Compressed pages, nested columns and the DELTA_* encodings are refused
+// BYTE_ARRAY, uncompressed and ZSTD-compressed pages.  Other codecs, nested columns and the DELTA_* encodings are refused
 // (SAILGPU_ERR_UNSUPPORTED): the caller keeps the CPU reader for those files.
+//
+// ZSTD chunks (Sail's writer default) are decompressed on the device first.  Page headers are stored uncompressed, so the host
+// walks them into a page table (where each page's frames start, how long they are, where the decompressed body goes) and
+// checks each page's first frame header.  One launch of parquet_zstd_decompress_kernel covers the compressed pages of every
+// column of the call, one warp per page (zstd.cuh), and builds a decompressed image of each chunk: every page's header bytes
+// followed by its decompressed body (the levels of a data page V2 are stored uncompressed and are copied as they are).  The
+// images are read back once, with a status per page, because the run-header walk below runs on the host; from there on a
+// ZSTD chunk is its image, already in HBM, and takes the uncompressed path.
 #include <cstring>
 
 #include "device.hpp"
 #include "h2d.hpp"
 #include "kernels.hpp"
+#include "zstd.cuh"
 
 namespace sg {
 
@@ -257,6 +266,37 @@ BufPtr upload_vec(Ctx* ctx, const void* p, size_t bytes) {
   return b;
 }
 
+// ---- ZSTD pages -> decompressed image ------------------------------------------------------------------------------------
+enum { CODEC_NONE = 0, CODEC_ZSTD = 6 };
+// one page of a ZSTD chunk: `copy` bytes (the page header, plus the levels of a data page V2, or the whole body of a V2 page
+// stored uncompressed) are copied as they are, then `comp` bytes of frames decompress to exactly `out` bytes
+struct ZPage { uint64_t src, dst; uint32_t copy, comp, out, pad; };
+
+constexpr int kZstdWarps = 4;      // warps per block; each warp owns a ZWork in shared memory and kBlockMax bytes of literal scratch
+
+__global__ void __launch_bounds__(kZstdWarps * 32) parquet_zstd_decompress_kernel(const uint8_t* __restrict__ src, const ZPage* __restrict__ pages, int n_pages,
+                                                                               uint8_t* __restrict__ image, uint8_t* __restrict__ lits, uint32_t* __restrict__ status) {
+  __shared__ zstd::ZWork work[kZstdWarps];
+  const int wid = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int gw = blockIdx.x * kZstdWarps + wid, nw = gridDim.x * kZstdWarps;
+  const zstd::WarpTeam team{lane};
+  uint8_t* my_lits = lits + (size_t)gw * zstd::kBlockMax;
+  for (int pg = gw; pg < n_pages; pg += nw) {
+    const ZPage P = pages[pg];
+    for (uint32_t i = lane; i < P.copy; i += 32) image[P.dst + i] = src[P.src + i];
+    int st = zstd::ZS_OK;
+    if (P.comp) st = zstd::decode_frames(team, &work[wid], src + P.src + P.copy, P.comp, image + P.dst + P.copy, P.out, my_lits);
+    if (lane == 0) status[pg] = (uint32_t)st;
+    __syncwarp();
+  }
+}
+
+std::string zstd_page_name(const Field& f, size_t page) { return "ZSTD page " + std::to_string(page) + " of column '" + f.name + "'"; }
+[[noreturn]] void zstd_page_fail(const Field& f, size_t page, int status) {
+  if (status == zstd::ZS_UNSUPPORTED) fail(SAILGPU_ERR_UNSUPPORTED, "parquet: " + zstd_page_name(f, page) + " needs a dictionary or holds a skippable frame");
+  fail(SAILGPU_ERR_INVALID, "parquet: " + zstd_page_name(f, page) + " is corrupt");
+}
+
 }  // namespace
 
 struct ParquetColumnDesc {      // mirrors sailgpu_parquet_column (include/sailgpu.h)
@@ -271,32 +311,91 @@ struct ColumnPlan {
   std::vector<Run> level_runs, index_runs;
   std::vector<Segment> segs;
   std::vector<uint64_t> str_off;
+  std::vector<std::pair<const uint8_t*, uint64_t>> bodies;     // every page body walked (decompressed for ZSTD), in page order
   int64_t dense = 0, dict_count = 0, dict_len = 0, n_pages = 0;
   const uint8_t* dict_bytes = nullptr;
   bool any_dict_page = false, any_plain_page = false, is_str = false;
   int out_width = 0;
 };
 
-ColumnPlan plan_parquet_column(const Field& f, const ParquetColumnDesc& c, int64_t n_rows) {
-  ColumnPlan P;
-
-  SG_CHECK(c.codec == 0, SAILGPU_ERR_UNSUPPORTED, "parquet: compressed pages are not decoded on the GPU path yet (column '" + f.name + "')");
+void check_parquet_column(const Field& f, const ParquetColumnDesc& c, int64_t n_rows) {
+  SG_CHECK(c.codec == CODEC_NONE || c.codec == CODEC_ZSTD, SAILGPU_ERR_UNSUPPORTED,
+           "parquet: only uncompressed and ZSTD pages are decoded on the GPU path (column '" + f.name + "' has codec " + std::to_string(c.codec) + ")");
   SG_CHECK(c.max_def_level == 0 || c.max_def_level == 1, SAILGPU_ERR_UNSUPPORTED, "parquet: nested / repeated columns are not supported (column '" + f.name + "')");
   SG_CHECK(c.num_values == n_rows, SAILGPU_ERR_INVALID, "parquet: column '" + f.name + "' has " + std::to_string(c.num_values) + " values for " + std::to_string(n_rows) + " rows");
   const int pt = c.physical_type;
   const bool is_str = f.type.is_string();
-  P.is_str = is_str;
   SG_CHECK(pt == PT_INT32 || pt == PT_INT64 || pt == PT_DOUBLE || pt == PT_FLBA || pt == PT_BYTE_ARRAY, SAILGPU_ERR_UNSUPPORTED,
            "parquet: physical type " + std::to_string(pt) + " (column '" + f.name + "')");
   SG_CHECK((pt == PT_BYTE_ARRAY) == is_str, SAILGPU_ERR_UNSUPPORTED, "parquet: BYTE_ARRAY columns decode to strings only (column '" + f.name + "')");
   SG_CHECK(f.type.id != TypeId::Utf8, SAILGPU_ERR_UNSUPPORTED, "parquet: strings decode to Utf8View (what Sail reads Parquet strings as: application.yaml:375-381)");
   const int out_width = is_str ? 16 : f.type.arrow_width();
-  P.out_width = out_width;
   SG_CHECK(out_width == 4 || out_width == 8 || out_width == 16, SAILGPU_ERR_UNSUPPORTED, "parquet: target type " + f.type.str());
   if (pt == PT_FLBA) SG_CHECK(f.type.is_decimal() && c.type_length >= 1 && c.type_length <= 16, SAILGPU_ERR_UNSUPPORTED, "parquet: FIXED_LEN_BYTE_ARRAY decodes to Decimal128 only");
   if (pt == PT_DOUBLE) SG_CHECK(f.type.id == TypeId::Float64, SAILGPU_ERR_UNSUPPORTED, "parquet: DOUBLE decodes to Float64");
   if (pt == PT_INT32) SG_CHECK(out_width == 4 || f.type.is_decimal(), SAILGPU_ERR_UNSUPPORTED, "parquet: INT32 decodes to 32-bit types or Decimal128");
   if (pt == PT_INT64) SG_CHECK(out_width == 8 || f.type.is_decimal(), SAILGPU_ERR_UNSUPPORTED, "parquet: INT64 decodes to 64-bit types or Decimal128");
+}
+
+// Walks the page headers of a ZSTD chunk into `pages` (source offsets from src_base, image offsets from dst_base) and checks
+// the first frame header of every page: magic number, no dictionary, a content size that fits the page.  Stops where
+// plan_parquet_column stops, once the data pages hold n_rows values.  Returns the length of the chunk's image.
+uint64_t plan_zstd_pages(const Field& f, const ParquetColumnDesc& c, int64_t n_rows, uint64_t src_base, uint64_t dst_base, std::vector<ZPage>* pages) {
+  const uint8_t* end = c.chunk + c.chunk_len;
+  TReader r{c.chunk, end};
+  uint64_t dst = dst_base;
+  int64_t rows_done = 0;
+  for (size_t idx = 0; r.p < end && rows_done < n_rows; ++idx) {
+    const uint8_t* start = r.p;
+    const PageHeader h = read_page_header(r);
+    SG_CHECK(h.compressed >= 0 && h.uncompressed >= 0 && r.p + h.compressed <= end, SAILGPU_ERR_INVALID, "parquet: page overruns its column chunk");
+    uint32_t keep = 0;                           // body bytes stored uncompressed
+    if (h.type == PAGE_DATA_V2) {
+      SG_CHECK(h.def_bytes >= 0 && h.rep_bytes >= 0, SAILGPU_ERR_INVALID, "parquet: negative level length");
+      keep = h.v2_compressed ? (uint32_t)h.def_bytes + (uint32_t)h.rep_bytes : (uint32_t)h.compressed;
+      SG_CHECK(h.v2_compressed || h.compressed == h.uncompressed, SAILGPU_ERR_INVALID, "parquet: uncompressed page V2 with two sizes");
+      SG_CHECK(keep <= (uint32_t)h.compressed && keep <= (uint32_t)h.uncompressed, SAILGPU_ERR_INVALID, "parquet: levels overrun their page");
+    }
+    const uint32_t hdr = (uint32_t)(r.p - start);
+    const ZPage p{src_base + (uint64_t)(start - c.chunk), dst, hdr + keep, (uint32_t)h.compressed - keep, (uint32_t)h.uncompressed - keep, 0};
+    if (p.comp) {
+      zstd::FrameHeader fh;
+      const int st = zstd::parse_frame_header(start + p.copy, p.comp, &fh);
+      if (st) zstd_page_fail(f, idx, st);
+      if (fh.has_content_size && fh.content_size > p.out) zstd_page_fail(f, idx, zstd::ZS_CORRUPT);
+    } else if (p.out) zstd_page_fail(f, idx, zstd::ZS_CORRUPT);
+    pages->push_back(p);
+    dst += (uint64_t)p.copy + p.out;
+    r.p += h.compressed;
+    if (h.type == PAGE_DATA || h.type == PAGE_DATA_V2) rows_done += h.num_values;
+  }
+  return dst - dst_base;
+}
+
+// The decompressed image of a ZSTD chunk, built on the host by the same decoder (sailgpu_parquet_inspect)
+std::vector<uint8_t> zstd_image_host(const Field& f, const ParquetColumnDesc& c, int64_t n_rows, uint64_t* image_len) {
+  std::vector<ZPage> pages;
+  *image_len = plan_zstd_pages(f, c, n_rows, 0, 0, &pages);
+  std::vector<uint8_t> img(*image_len + 64, 0), lits(zstd::kBlockMax);
+  auto work = std::make_unique<zstd::ZWork>();
+  for (size_t i = 0; i < pages.size(); ++i) {
+    const ZPage& p = pages[i];
+    memcpy(img.data() + p.dst, c.chunk + p.src, p.copy);
+    if (!p.comp) continue;
+    const int st = zstd::decode_frames(zstd::SerialTeam{}, work.get(), c.chunk + p.src + p.copy, p.comp, img.data() + p.dst + p.copy, p.out, lits.data());
+    if (st) zstd_page_fail(f, i, st);
+  }
+  return img;
+}
+
+// `c` describes the chunk as stored when it is uncompressed, and its decompressed image when its codec is ZSTD
+ColumnPlan plan_parquet_column(const Field& f, const ParquetColumnDesc& c, int64_t n_rows) {
+  ColumnPlan P;
+  check_parquet_column(f, c, n_rows);
+  const bool is_str = f.type.is_string();
+  P.is_str = is_str;
+  P.out_width = is_str ? 16 : f.type.arrow_width();
+  const bool image = c.codec == CODEC_ZSTD;
 
   // ---- host: page headers and run headers -----------------------------------------------------------------------
   const uint8_t* base = c.chunk; const uint8_t* end = c.chunk + c.chunk_len;
@@ -309,13 +408,16 @@ ColumnPlan plan_parquet_column(const Field& f, const ParquetColumnDesc& c, int64
   TReader r{base, end};
   while (r.p < end && rows_done < n_rows) {
     const PageHeader h = read_page_header(r);
-    SG_CHECK(h.compressed == h.uncompressed, SAILGPU_ERR_UNSUPPORTED, "parquet: compressed page in column '" + f.name + "'");
-    const uint8_t* body = r.p; const uint8_t* body_end = body + h.compressed;
+    if (!image) SG_CHECK(h.compressed == h.uncompressed, SAILGPU_ERR_UNSUPPORTED, "parquet: compressed page in column '" + f.name + "'");
+    const int64_t body_len = image ? h.uncompressed : h.compressed;      // an image holds every body decompressed
+    SG_CHECK(body_len >= 0, SAILGPU_ERR_INVALID, "parquet: negative page size");
+    const uint8_t* body = r.p; const uint8_t* body_end = body + body_len;
     SG_CHECK(body_end <= end, SAILGPU_ERR_INVALID, "parquet: page overruns its column chunk");
     r.p = body_end;
+    P.bodies.emplace_back(body, (uint64_t)body_len);
     if (h.type == PAGE_DICT) {
       SG_CHECK(h.encoding == ENC_PLAIN || h.encoding == ENC_PLAIN_DICT, SAILGPU_ERR_UNSUPPORTED, "parquet: dictionary page encoding " + std::to_string(h.encoding));
-      have_dict = true; dict_count = h.num_values; dict_bytes = body; dict_len = h.compressed;
+      have_dict = true; dict_count = h.num_values; dict_bytes = body; dict_len = body_len;
       continue;
     }
     if (h.type != PAGE_DATA && h.type != PAGE_DATA_V2) continue;       // index pages etc.
@@ -370,7 +472,8 @@ ColumnPlan plan_parquet_column(const Field& f, const ParquetColumnDesc& c, int64
   return P;
 }
 
-DevColumn decode_parquet_column(Ctx* ctx, const Field& f, const ParquetColumnDesc& c, int64_t n_rows) {
+// dimage: for a ZSTD chunk, its image in HBM (c describes the host copy of that image); `image_buf` holds it
+DevColumn decode_parquet_column(Ctx* ctx, const Field& f, const ParquetColumnDesc& c, int64_t n_rows, const uint8_t* dimage = nullptr, BufPtr image_buf = nullptr) {
   ColumnPlan P = plan_parquet_column(f, c, n_rows);
   const uint8_t* base = c.chunk;
   const int pt = c.physical_type;
@@ -384,13 +487,14 @@ DevColumn decode_parquet_column(Ctx* ctx, const Field& f, const ParquetColumnDes
   const bool any_dict_page = P.any_dict_page, any_plain_page = P.any_plain_page;
   // ---- device ---------------------------------------------------------------------------------------------------------
   DevColumn col; col.type = f.type; col.length = n_rows;
-  BufPtr dchunk = dev_alloc(ctx, (size_t)c.chunk_len + 64);
-  {
+  BufPtr dchunk = image_buf;
+  if (!dimage) {
+    dchunk = dev_alloc(ctx, (size_t)c.chunk_len + 64);
     HostStager st(ctx);
     st.add_raw(dchunk->ptr, c.chunk, (size_t)c.chunk_len);
     st.flush();
   }
-  const uint8_t* dbase = static_cast<const uint8_t*>(dchunk->ptr);
+  const uint8_t* dbase = dimage ? dimage : static_cast<const uint8_t*>(dchunk->ptr);
   BufPtr err = dev_alloc_zero(ctx, 8);
   auto expand = [&](const std::vector<Run>& runs, int64_t n) -> BufPtr {
     BufPtr out = dev_alloc(ctx, (size_t)n * 4 + 16);
@@ -470,17 +574,106 @@ DevColumn decode_parquet_column(Ctx* ctx, const Field& f, const ParquetColumnDes
   return col;
 }
 
-// host-only summary of a column plan (tests/test_parquet_plan.py pins the page / run walking against pyarrow's own metadata)
+// One row group: the compressed pages of every ZSTD column go through one decompression launch and one read-back, then each
+// column is decoded (a ZSTD column from its image, an uncompressed one as stored).
+void decode_parquet_row_group(Ctx* ctx, const Schema& schema, const std::vector<ParquetColumnDesc>& cols, int64_t n_rows, DevBatch* b) {
+  const size_t nc = cols.size();
+  std::vector<ZPage> pages;
+  std::vector<size_t> first_page(nc + 1, 0);
+  std::vector<uint64_t> src_off(nc, 0), img_off(nc, 0), img_len(nc, 0);
+  uint64_t src_total = 0, img_total = 0, out_bytes = 0;
+  for (size_t i = 0; i < nc; ++i) {
+    first_page[i] = pages.size();
+    check_parquet_column(schema[i], cols[i], n_rows);
+    if (cols[i].codec != CODEC_ZSTD) continue;
+    src_off[i] = src_total; img_off[i] = img_total;
+    img_len[i] = plan_zstd_pages(schema[i], cols[i], n_rows, src_total, img_total, &pages);
+    src_total += cols[i].chunk_len;
+    img_total = (img_total + img_len[i] + 63) & ~(uint64_t)63;
+  }
+  first_page[nc] = pages.size();
+  for (const ZPage& p : pages) out_bytes += p.out;
+  ctx->parquet_zstd = Ctx::ParquetZstd{};
+  BufPtr dimg;
+  std::vector<uint8_t> himg;
+  const size_t status_bytes = (pages.size() * 4 + 255) & ~(size_t)255;     // per-page status ahead of the images
+  bool any_zstd = false;
+  for (const ParquetColumnDesc& c : cols) any_zstd |= c.codec == CODEC_ZSTD;
+  if (any_zstd) {                                // (a chunk of an empty row group has no page to decompress, but still an image)
+    dimg = dev_alloc(ctx, status_bytes + (size_t)img_total + 64);
+    himg.assign(status_bytes + (size_t)img_total + 64, 0);
+  }
+  if (!pages.empty()) {
+    SG_CHECK(pages.size() < (size_t)INT32_MAX, SAILGPU_ERR_UNSUPPORTED, "parquet: too many pages in one call");
+    BufPtr dsrc = dev_alloc(ctx, (size_t)src_total + 64);
+    {
+      HostStager st(ctx);
+      for (size_t i = 0; i < nc; ++i)
+        if (cols[i].codec == CODEC_ZSTD && cols[i].chunk_len) st.add_raw(static_cast<uint8_t*>(dsrc->ptr) + src_off[i], cols[i].chunk, (size_t)cols[i].chunk_len);
+      st.flush();
+    }
+    BufPtr dpages = upload_vec(ctx, pages.data(), pages.size() * sizeof(ZPage));
+    int per_sm = 0;
+    SG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, parquet_zstd_decompress_kernel, kZstdWarps * 32, 0));
+    const int blocks = (int)std::min<int64_t>(((int64_t)pages.size() + kZstdWarps - 1) / kZstdWarps, (int64_t)std::max(per_sm, 1) * ctx->sm_count);
+    BufPtr lits = dev_alloc(ctx, (size_t)blocks * kZstdWarps * zstd::kBlockMax);
+    uint8_t* dbase = static_cast<uint8_t*>(dimg->ptr);
+    cudaEvent_t ev[3];
+    for (auto& e : ev) SG_CUDA(cudaEventCreate(&e));
+    SG_CUDA(cudaEventRecord(ev[0], ctx->stream));
+    parquet_zstd_decompress_kernel<<<blocks, kZstdWarps * 32, 0, ctx->stream>>>(static_cast<const uint8_t*>(dsrc->ptr), static_cast<const ZPage*>(dpages->ptr), (int)pages.size(),
+                                                                            dbase + status_bytes, static_cast<uint8_t*>(lits->ptr), reinterpret_cast<uint32_t*>(dbase));
+    SG_CUDA(cudaGetLastError());
+    SG_CUDA(cudaEventRecord(ev[1], ctx->stream));
+    SG_CUDA(cudaMemcpyAsync(himg.data(), dbase, status_bytes + (size_t)img_total, cudaMemcpyDeviceToHost, ctx->stream));
+    SG_CUDA(cudaEventRecord(ev[2], ctx->stream));
+    stream_sync(ctx);        // the run-header walk reads the images on the host
+    ctx->d2h_bytes += status_bytes + img_total;
+    Ctx::ParquetZstd& s = ctx->parquet_zstd;
+    s.pages = pages.size(); s.out_bytes = out_bytes; s.image_bytes = img_total;
+    SG_CUDA(cudaEventElapsedTime(&s.decompress_ms, ev[0], ev[1]));
+    SG_CUDA(cudaEventElapsedTime(&s.readback_ms, ev[1], ev[2]));
+    for (auto& e : ev) cudaEventDestroy(e);
+    const uint32_t* status = reinterpret_cast<const uint32_t*>(himg.data());
+    for (size_t i = 0; i < nc; ++i)
+      for (size_t k = first_page[i]; k < first_page[i + 1]; ++k)
+        if (status[k]) zstd_page_fail(schema[i], k - first_page[i], (int)status[k]);
+  }
+  for (size_t i = 0; i < nc; ++i) {
+    if (cols[i].codec != CODEC_ZSTD) { b->cols.push_back(decode_parquet_column(ctx, schema[i], cols[i], n_rows)); continue; }
+    ParquetColumnDesc d = cols[i];
+    d.chunk = himg.data() + status_bytes + img_off[i]; d.chunk_len = img_len[i];
+    b->cols.push_back(decode_parquet_column(ctx, schema[i], d, n_rows, static_cast<const uint8_t*>(dimg->ptr) + status_bytes + img_off[i], dimg));
+  }
+}
+
+// FNV-1a, 64 bits
+static uint64_t fnv1a(uint64_t h, const uint8_t* p, uint64_t n) {
+  for (uint64_t i = 0; i < n; ++i) { h ^= p[i]; h *= 0x100000001b3ull; }
+  return h;
+}
+
+// host-only summary of a column plan (tests/test_parquet_plan.py pins the page / run walking against pyarrow's own metadata);
+// a ZSTD chunk is decompressed on the host by the decoder the device runs
 std::string parquet_plan_summary(const Field& f, const ParquetColumnDesc& c, int64_t n_rows) {
-  ColumnPlan P = plan_parquet_column(f, c, n_rows);
+  std::vector<uint8_t> img;
+  ParquetColumnDesc d = c;
+  if (c.codec == CODEC_ZSTD) {
+    check_parquet_column(f, c, n_rows);
+    img = zstd_image_host(f, c, n_rows, &d.chunk_len);
+    d.chunk = img.data();
+  }
+  ColumnPlan P = plan_parquet_column(f, d, n_rows);
   int64_t level_vals = 0, index_vals = 0;
   for (auto& r : P.level_runs) level_vals += r.count;
   for (auto& r : P.index_runs) index_vals += r.count;
-  char b[512];
+  uint64_t body_bytes = 0, body_hash = 0xcbf29ce484222325ull;
+  for (auto& s : P.bodies) { body_bytes += s.second; body_hash = fnv1a(body_hash, s.first, s.second); }
+  char b[640];
   snprintf(b, sizeof b, "{\"pages\":%lld,\"dense\":%lld,\"dict_count\":%lld,\"level_values\":%lld,\"index_values\":%lld,\"level_runs\":%zu,\"index_runs\":%zu,"
-                        "\"plain_strings\":%zu,\"dict_pages\":%d,\"plain_pages\":%d}",
+                        "\"plain_strings\":%zu,\"dict_pages\":%d,\"plain_pages\":%d,\"body_bytes\":%llu,\"body_fnv1a\":%llu}",
            (long long)P.n_pages, (long long)P.dense, (long long)P.dict_count, (long long)level_vals, (long long)index_vals, P.level_runs.size(), P.index_runs.size(),
-           P.str_off.size(), P.any_dict_page ? 1 : 0, P.any_plain_page ? 1 : 0);
+           P.str_off.size(), P.any_dict_page ? 1 : 0, P.any_plain_page ? 1 : 0, (unsigned long long)body_bytes, (unsigned long long)body_hash);
   return b;
 }
 

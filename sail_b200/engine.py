@@ -79,6 +79,7 @@ def lib():
         L.sailgpu_jit_precompile.restype = i64
         L.sailgpu_parquet_decode.argtypes = [vp, vp, vp, i32, i64, vp]
         L.sailgpu_parquet_inspect.argtypes = [vp, vp, i32, i64, i32, ctypes.c_char_p, ctypes.c_size_t]
+        L.sailgpu_parquet_stats.argtypes = [vp, ctypes.c_char_p, ctypes.c_size_t]
         L.sailgpu_op_push.argtypes = [vp, i32, vp]
         L.sailgpu_op_push_device.argtypes = [vp, i32, vp]
         L.sailgpu_op_finish_input.argtypes = [vp, i32]
@@ -545,6 +546,17 @@ def parquet_inspect(file_bytes, column: int, row_group: int = 0, columns: list |
     del buf
     if rc != 0:
         raise SailGpuError(rc, out.value.decode())
+    return json.loads(out.value.decode())
+
+
+def parquet_stats(ctx: Context | None = None) -> dict:
+    """What the last parquet_decode on `ctx` spent on ZSTD pages: page count, decompressed bytes, image bytes read back, and the
+    device milliseconds of the decompression launch and of the read-back."""
+    ctx = ctx or default_context()
+    out = ctypes.create_string_buffer(512)
+    rc = lib().sailgpu_parquet_stats(ctx._h, out, 512)
+    if rc != 0:
+        raise SailGpuError(rc, lib().sailgpu_ctx_last_error(None).decode())
     return json.loads(out.value.decode())
 
 
