@@ -253,18 +253,21 @@ struct Emitter {
       ops.push_back(A.accs[j].op); words.push_back(A.accs[j].word); seen.push_back(A.accs[j].track_seen);
       modes.push_back(A.accs[j].op == ACC_COUNT ? 0 : A.accs[j].vkind == K_I64 ? (J.small_acc[j] ? 3 : 1) : 2);
     }
+    // the key in registers is padded to the dictionary's HOT_KEY_WORDS words (those tiers compare and fingerprint four words)
+    const int key_regs = std::max(A.key_words, HOT_KEY_WORDS);
     o << "  static constexpr int N_KEYS = " << A.n_keys << ", KEY_WORDS = " << A.key_words << ", N_ACCS = " << A.n_accs << ", ENTRY_WORDS = " << (2 + A.key_words + A.acc_words)
       << ", HOT_G = " << std::max(hot_g, 1) << ", AGG_TIER = " << tier << ";\n";
+    o << "  using Key = JitKey<" << key_regs << ">;\n";
     o << "  static __device__ __forceinline__ constexpr int acc_op(int j) { return " << chain(ops) << "; }\n";
     o << "  static __device__ __forceinline__ constexpr int acc_word(int j) { return " << chain(words) << "; }\n";
     o << "  static __device__ __forceinline__ constexpr int acc_seen(int j) { return " << chain(seen) << "; }\n";
     o << "  static __device__ __forceinline__ constexpr int reg_mode(int j) { return " << chain(modes) << "; }\n";
     // key words
     std::ostringstream kwf, khf, kef;
-    kwf << "  static __device__ __forceinline__ void key_words(const Row& o, uint64_t (&kw)[MAX_KEY_WORDS]) {\n";
-    khf << "  static __device__ __forceinline__ uint64_t key_hash(const uint64_t (&kw)[MAX_KEY_WORDS]) {\n    uint64_t h = 0x243F6A8885A308D3ull;\n";
-    kef << "  static __device__ __forceinline__ bool keys_equal(const uint64_t* a, const uint64_t (&kw)[MAX_KEY_WORDS]) {\n    bool eq = true;\n";
-    if (A.has_null_word) { kwf << "    uint64_t nm = 0;\n"; kef << "    eq = eq && a[0] == kw[0];\n"; }
+    kwf << "  static __device__ __forceinline__ void key_words(const Row& o, Key& k) {\n";
+    khf << "  static __device__ __forceinline__ uint64_t key_hash(const Key& k) {\n    uint64_t h = 0x243F6A8885A308D3ull;\n";
+    kef << "  static __device__ __forceinline__ bool keys_equal(const uint64_t* a, const Key& k) {\n    bool eq = true;\n";
+    if (A.has_null_word) { kwf << "    uint64_t nm = 0;\n"; kef << "    eq = eq && a[0] == k.w[0];\n"; }
     int w = A.has_null_word ? 1 : 0;
     for (int i = 0; i < A.n_keys; ++i) {
       const KeyDesc& k = A.keys[i];
@@ -273,15 +276,15 @@ struct Emitter {
       std::string nul = "false";
       if (k.valid_slot != NO_SLOT) { nul = "!o." + field(k.valid_slot, K_B, 1); kwf << "    if (" << nul << ") nm |= " << (1ull << i) << "ull;\n"; }
       if (k.width == 16) {
-        if (kk == K_V16) kwf << "    kw[" << w << "] = " << nul << " ? 0ull : " << f << ".x; kw[" << w + 1 << "] = " << nul << " ? 0ull : " << f << ".y;\n";
-        else kwf << "    kw[" << w << "] = " << nul << " ? 0ull : i128_lo(" << f << "); kw[" << w + 1 << "] = " << nul << " ? 0ull : i128_hi(" << f << ");\n";
-        const std::string v = "mkv16(kw[" + std::to_string(w) + "], kw[" + std::to_string(w + 1) + "])";
+        if (kk == K_V16) kwf << "    k.w[" << w << "] = " << nul << " ? 0ull : " << f << ".x; k.w[" << w + 1 << "] = " << nul << " ? 0ull : " << f << ".y;\n";
+        else kwf << "    k.w[" << w << "] = " << nul << " ? 0ull : i128_lo(" << f << "); k.w[" << w + 1 << "] = " << nul << " ? 0ull : i128_hi(" << f << ");\n";
+        const std::string v = "mkv16(k.w[" + std::to_string(w) + "], k.w[" + std::to_string(w + 1) + "])";
         if (k.is_view) {
           khf << "    h = mix64(h ^ view_hash(" << v << "));\n";
           kef << "    eq = eq && view_equal(mkv16(a[" << w << "], a[" << w + 1 << "]), " << v << ");\n";
         } else {
-          khf << "    h = mix64(h ^ mix64(kw[" << w << "] ^ mix64(kw[" << w + 1 << "])));\n";
-          kef << "    eq = eq && a[" << w << "] == kw[" << w << "] && a[" << w + 1 << "] == kw[" << w + 1 << "];\n";
+          khf << "    h = mix64(h ^ mix64(k.w[" << w << "] ^ mix64(k.w[" << w + 1 << "])));\n";
+          kef << "    eq = eq && a[" << w << "] == k.w[" << w << "] && a[" << w + 1 << "] == k.w[" << w + 1 << "];\n";
         }
         w += 2;
       } else {
@@ -291,14 +294,14 @@ struct Emitter {
         else if (kk == K_I32) bits = "(uint64_t)(uint32_t)" + f;
         else if (kk == K_B) bits = "(" + f + " ? 1ull : 0ull)";
         else throw Unsupported{"group key kind"};
-        kwf << "    kw[" << w << "] = " << nul << " ? 0ull : " << bits << ";\n";
-        khf << "    h = mix64(h ^ kw[" << w << "]);\n";
-        kef << "    eq = eq && a[" << w << "] == kw[" << w << "];\n";
+        kwf << "    k.w[" << w << "] = " << nul << " ? 0ull : " << bits << ";\n";
+        khf << "    h = mix64(h ^ k.w[" << w << "]);\n";
+        kef << "    eq = eq && a[" << w << "] == k.w[" << w << "];\n";
         w += 1;
       }
     }
-    if (A.has_null_word) { kwf << "    kw[0] = nm;\n"; khf << "    h = mix64(h ^ kw[0]);\n"; }
-    for (int z = w; z < MAX_KEY_WORDS; ++z) kwf << "    kw[" << z << "] = 0ull;\n";
+    if (A.has_null_word) { kwf << "    k.w[0] = nm;\n"; khf << "    h = mix64(h ^ k.w[0]);\n"; }
+    for (int z = w; z < key_regs; ++z) kwf << "    k.w[" << z << "] = 0ull;\n";
     kwf << "  }\n"; khf << "    return h;\n  }\n"; kef << "    return eq;\n  }\n";
     o << kwf.str() << khf.str() << kef.str();
     // accumulator inputs

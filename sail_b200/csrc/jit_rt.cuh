@@ -15,6 +15,11 @@
 
 namespace sg {
 
+// A group key in registers: the packed key words, padded with zeros to HOT_KEY_WORDS (G::Key, jit.cu).  Indexed only by
+// constants and passed by value, so that it stays in registers -- never a local-memory array.
+template <int N> struct JitKey { uint64_t w[N]; };
+using JitHotKey = JitKey<HOT_KEY_WORDS>;
+
 template <int I> struct IC { static constexpr int value = I; __device__ constexpr operator int() const { return I; } };
 template <int I, int N, class F> __device__ __forceinline__ void static_for(F&& f) {
   if constexpr (I < N) { f(IC<I>{}); static_for<I + 1, N>(f); }
@@ -132,10 +137,10 @@ __device__ __forceinline__ T jit_gather(uint64_t base, int64_t row) {
 // global group table (layout and protocol of pipeline.cu::agg_find_or_insert, constants from G)
 // ================================================================================================
 template <class G>
-__device__ __forceinline__ uint64_t* jit_find_or_insert(const AggParams& A, const uint64_t (&kw)[MAX_KEY_WORDS], uint64_t h, uint32_t* err) {
+__device__ __forceinline__ uint64_t* jit_find_or_insert(const AggParams& A, const typename G::Key& kw, uint64_t h, uint32_t* err) {
   if constexpr (G::KEY_WORDS == 1) {
     if (A.direct_key) {          // direct-key protocol (vm.h): one CAS on the key word, no fence, no state word
-      const unsigned long long k = kw[0];
+      const unsigned long long k = kw.w[0];
       if (k == DIRECT_EMPTY_KEY) {
         uint64_t* e = reinterpret_cast<uint64_t*>(A.table) + (A.capacity_mask + 1) * G::ENTRY_WORDS;
         if (*reinterpret_cast<volatile unsigned long long*>(e) == 0ull && atomicCAS(reinterpret_cast<unsigned long long*>(e), 0ull, h | 1ull) == 0ull) atomicAdd(A.n_groups, 1ull);
@@ -175,7 +180,7 @@ __device__ __forceinline__ uint64_t* jit_find_or_insert(const AggParams& A, cons
         e[0] = h;
         e[1] = 0;
 #pragma unroll
-        for (int w = 0; w < G::KEY_WORDS; ++w) e[2 + w] = kw[w];
+        for (int w = 0; w < G::KEY_WORDS; ++w) e[2 + w] = kw.w[w];
         static_for<0, G::N_ACCS>([&](auto Jc) { constexpr int J = decltype(Jc)::value;
 #pragma unroll
           for (int w = 0; w < acc_words_of(G::acc_op(J)); ++w) e[2 + G::KEY_WORDS + G::acc_word(J) + w] = acc_identity(G::acc_op(J), w);
@@ -209,7 +214,7 @@ __device__ __forceinline__ uint64_t* jit_find_or_insert(const AggParams& A, cons
 }
 
 template <class G>
-__device__ __forceinline__ uint64_t* jit_find_or_insert_warp(const AggParams& A, const uint64_t (&kw)[MAX_KEY_WORDS], uint64_t h, bool need, uint32_t* err) {
+__device__ __forceinline__ uint64_t* jit_find_or_insert_warp(const AggParams& A, const typename G::Key& kw, uint64_t h, bool need, uint32_t* err) {
   const unsigned lane = threadIdx.x & 31;
   const unsigned long long probe = need ? h : (0xFFFFFFFF00000000ull | lane);
   const unsigned peers = __match_any_sync(0xFFFFFFFFu, probe);
@@ -261,20 +266,20 @@ template <class G> __device__ __forceinline__ JitHot jit_hot(uint8_t* scratch) {
 }
 template <class G> constexpr int jit_aw() { return 1 + 2 * G::N_ACCS; }     // per (warp, group): seen word + {lo, hi} per accumulator
 
-__device__ __forceinline__ uint32_t jit_fp(const uint64_t (&kw)[MAX_KEY_WORDS]) {
-  uint32_t fp = fold32(kw[0]);
-  fp = __funnelshift_l(fp, fp, 7) ^ fold32(kw[1]);
-  fp = __funnelshift_l(fp, fp, 7) ^ fold32(kw[2]);
-  fp = __funnelshift_l(fp, fp, 7) ^ fold32(kw[3]);
+__device__ __forceinline__ uint32_t jit_fp(const JitHotKey& kw) {
+  uint32_t fp = fold32(kw.w[0]);
+  fp = __funnelshift_l(fp, fp, 7) ^ fold32(kw.w[1]);
+  fp = __funnelshift_l(fp, fp, 7) ^ fold32(kw.w[2]);
+  fp = __funnelshift_l(fp, fp, 7) ^ fold32(kw.w[3]);
   return fp;
 }
-__device__ __forceinline__ bool jit_dict_verify(const JitHot& H, int g, const uint64_t (&kw)[MAX_KEY_WORDS]) {
+__device__ __forceinline__ bool jit_dict_verify(const JitHot& H, int g, const JitHotKey& kw) {
   const ulonglong2* hk = reinterpret_cast<const ulonglong2*>(H.keys + g * HOT_KEY_WORDS);
   const ulonglong2 a = hk[0], b = hk[1];
-  return ((a.x ^ kw[0]) | (a.y ^ kw[1]) | (b.x ^ kw[2]) | (b.y ^ kw[3])) == 0ull;
+  return ((a.x ^ kw.w[0]) | (a.y ^ kw.w[1]) | (b.x ^ kw.w[2]) | (b.y ^ kw.w[3])) == 0ull;
 }
 template <int CAP>
-__device__ __forceinline__ int jit_dict_lookup(const JitHot& H, int n, const uint64_t (&kw)[MAX_KEY_WORDS], uint32_t fp) {
+__device__ __forceinline__ int jit_dict_lookup(const JitHot& H, int n, const JitHotKey& kw, uint32_t fp) {
   const uint4 f0 = *reinterpret_cast<const uint4*>(H.fp32);
   if (n > 0 && f0.x == fp && jit_dict_verify(H, 0, kw)) return 0;
   if (n > 1 && f0.y == fp && jit_dict_verify(H, 1, kw)) return 1;
@@ -290,9 +295,10 @@ __device__ __forceinline__ int jit_dict_lookup(const JitHot& H, int n, const uin
   return -1;
 }
 // warp-collective: lanes with `want` find their key in the dictionary or append it while there is room (CAP entries);
-// returns the group id or -1 (dictionary full)
+// returns the group id or -1 (dictionary full).  Out of line (it runs while the dictionary grows), so H and the key are
+// passed by value: a reference would keep them in local memory in the caller, stored on every tile.
 template <int CAP>
-__device__ __noinline__ int jit_dict_add(JitSmem* sm, const JitHot& H, bool want, const uint64_t (&kw)[MAX_KEY_WORDS], uint32_t fp) {
+__device__ __noinline__ int jit_dict_add(JitSmem* sm, const JitHot H, bool want, const JitHotKey kw, uint32_t fp) {
   const int lane = threadIdx.x & 31;
   int g = -1;
   bool gave_up = false;
@@ -308,7 +314,7 @@ __device__ __noinline__ int jit_dict_add(JitSmem* sm, const JitHot& H, bool want
       if (g < 0) {
         if (n < CAP) {
 #pragma unroll
-          for (int w = 0; w < HOT_KEY_WORDS; ++w) H.keys[n * HOT_KEY_WORDS + w] = kw[w];
+          for (int w = 0; w < HOT_KEY_WORDS; ++w) H.keys[n * HOT_KEY_WORDS + w] = kw.w[w];
           H.fp32[n] = fp;
           H.entry[n] = 0;
           sts_release_u32(&sm->dict_n, (uint32_t)(n + 1));
@@ -329,12 +335,12 @@ __device__ __noinline__ int jit_dict_add(JitSmem* sm, const JitHot& H, bool want
 }
 
 template <class G>
-__device__ __noinline__ uint64_t* jit_hot_entry(const KernelArgs& K, const JitHot& H, int g) {
+__device__ __noinline__ uint64_t* jit_hot_entry(const KernelArgs& K, const JitHot H, int g) {
   uint64_t* e = reinterpret_cast<uint64_t*>(*reinterpret_cast<volatile uint64_t*>(H.entry + g));
   if (e) return e;
-  uint64_t kw[MAX_KEY_WORDS];
+  typename G::Key kw;
 #pragma unroll
-  for (int w = 0; w < MAX_KEY_WORDS; ++w) kw[w] = (w < G::KEY_WORDS && w < HOT_KEY_WORDS) ? H.keys[g * HOT_KEY_WORDS + w] : 0ull;
+  for (int w = 0; w < HOT_KEY_WORDS; ++w) kw.w[w] = w < G::KEY_WORDS ? H.keys[g * HOT_KEY_WORDS + w] : 0ull;
   e = jit_find_or_insert<G>(K.aux[0].agg, kw, G::key_hash(kw), K.P[0].error_flag);
   H.entry[g] = reinterpret_cast<uint64_t>(e);       // benign race: every writer stores the same pointer
   return e;
@@ -376,7 +382,7 @@ __device__ __forceinline__ void jit_cold_rows(const KernelArgs& K, const typenam
   for (int k = 0; k < G::RPT; ++k) {
     hh[k] = 0;
     if (rows[k].live && gid[k] < 0) {
-      uint64_t kw[MAX_KEY_WORDS];
+      typename G::Key kw;
       G::key_words(rows[k], kw);
       hh[k] = G::key_hash(kw);
       const uint64_t idx = hh[k] & A.capacity_mask;
@@ -388,7 +394,7 @@ __device__ __forceinline__ void jit_cold_rows(const KernelArgs& K, const typenam
   for (int k = 0; k < G::RPT; ++k) {
     const bool cold = rows[k].live && gid[k] < 0;
     if (__any_sync(0xFFFFFFFFu, cold)) {
-      uint64_t kw[MAX_KEY_WORDS];
+      typename G::Key kw;
       G::key_words(rows[k], kw);
       uint64_t* e = jit_find_or_insert_warp<G>(A, kw, hh[k], cold, K.P[0].error_flag);
       // Rows of one group that sit in the same warp (clustered inputs: the 1-7 lineitems of an order are neighbours) are combined
@@ -465,6 +471,7 @@ constexpr int JIT_REG_FLUSH = 224;
 // tier 2: counts / integer / decimal sums, first REG_GROUPS groups in registers
 template <class G>
 __device__ __forceinline__ void jit_agg_reg_tile(const KernelArgs& K, const typename G::Row (&rows)[G::RPT], JitSmem* sm, uint8_t* scratch, JitAggRegs<G>& R) {
+  static_assert(sizeof(typename G::Key) == sizeof(JitHotKey), "dictionary tiers hold keys of at most HOT_KEY_WORDS words");
   const JitHot H = jit_hot<G>(scratch);
   int gid[G::RPT];
   uint32_t fpv[G::RPT];
@@ -476,7 +483,7 @@ __device__ __forceinline__ void jit_agg_reg_tile(const KernelArgs& K, const type
   for (int k = 0; k < G::RPT; ++k) {
     gid[k] = -1; fpv[k] = 0;
     if (rows[k].live) {
-      uint64_t kw[MAX_KEY_WORDS];
+      typename G::Key kw;
       G::key_words(rows[k], kw);
       fpv[k] = jit_fp(kw);
       gid[k] = jit_dict_lookup<REG_GROUPS>(H, n0, kw, fpv[k]);
@@ -488,7 +495,7 @@ __device__ __forceinline__ void jit_agg_reg_tile(const KernelArgs& K, const type
     for (int k = 0; k < G::RPT; ++k) {
       const bool want = rows[k].live && gid[k] < 0;
       if (__any_sync(0xFFFFFFFFu, want)) {
-        uint64_t kw[MAX_KEY_WORDS];
+        typename G::Key kw;
         G::key_words(rows[k], kw);
         const int g = jit_dict_add<REG_GROUPS>(sm, H, want, kw, fpv[k]);
         if (want) gid[k] = g;
@@ -545,6 +552,7 @@ __device__ __forceinline__ void jit_agg_reg_tile(const KernelArgs& K, const type
 // tier 1: any accumulator mix, up to HOT_G groups, per-warp accumulators in shared memory (warp-shuffle reductions)
 template <class G>
 __device__ __forceinline__ void jit_agg_dict_tile(const KernelArgs& K, const typename G::Row (&rows)[G::RPT], JitSmem* sm, uint8_t* scratch) {
+  static_assert(sizeof(typename G::Key) == sizeof(JitHotKey), "dictionary tiers hold keys of at most HOT_KEY_WORDS words");
   const JitHot H = jit_hot<G>(scratch);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   int gid[G::RPT];
@@ -555,7 +563,7 @@ __device__ __forceinline__ void jit_agg_dict_tile(const KernelArgs& K, const typ
   for (int k = 0; k < G::RPT; ++k) {
     gid[k] = -1; fpv[k] = 0;
     if (rows[k].live) {
-      uint64_t kw[MAX_KEY_WORDS];
+      typename G::Key kw;
       G::key_words(rows[k], kw);
       fpv[k] = jit_fp(kw);
       gid[k] = jit_dict_lookup<G::HOT_G>(H, n0, kw, fpv[k]);
@@ -567,7 +575,7 @@ __device__ __forceinline__ void jit_agg_dict_tile(const KernelArgs& K, const typ
     for (int k = 0; k < G::RPT; ++k) {
       const bool want = rows[k].live && gid[k] < 0;
       if (__any_sync(0xFFFFFFFFu, want)) {
-        uint64_t kw[MAX_KEY_WORDS];
+        typename G::Key kw;
         G::key_words(rows[k], kw);
         const int g = jit_dict_add<G::HOT_G>(sm, H, want, kw, fpv[k]);
         if (want) gid[k] = g;
