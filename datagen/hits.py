@@ -129,3 +129,17 @@ def hits(n: int, seed: int = 0, strings: str = "view", columns=None) -> pa.Table
         else:
             arrays.append(pa.array(np.ascontiguousarray(v)))
     return pa.table(arrays, names=names)
+
+
+def stored(table: pa.Table) -> pa.Table:
+    """`hits(n)` with the column types the reference's hits.parquet stores (test_clickbench.py:11-119): strings as `binary`
+    (Parquet BYTE_ARRAY without a UTF8 annotation) and EventDate as UInt16 days since the epoch (INT32 annotated INT(16, unsigned));
+    the Int16 / Int32 / Int64 columns are stored as they are.  sail_b200.clickbench.view turns the stored types back into `hits`'s."""
+    arrays = []
+    for f, c in zip(table.schema, table.columns):
+        if pa.types.is_string_view(f.type) or pa.types.is_string(f.type):
+            c = c.cast(pa.binary())
+        elif pa.types.is_date32(f.type):
+            c = c.cast(pa.int32()).cast(pa.uint16())
+        arrays.append(c)
+    return pa.table(arrays, names=table.schema.names)

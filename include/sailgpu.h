@@ -189,7 +189,11 @@ SAILGPU_API int32_t sailgpu_spec_validate(const char* spec_json, size_t spec_len
  * exactly as stored in the file (dictionary page first) plus what the footer says about it; the chunk crosses PCIe as stored and is
  * decoded on the device (page headers and RLE run headers are walked on the host, every value is produced by a GPU thread).
  * `schema` names the Arrow type each column decodes to (Int32/Date32, Int64, Float64, Decimal128 from FIXED_LEN_BYTE_ARRAY /
- * INT32 / INT64, Utf8View from BYTE_ARRAY).  Covered: data pages V1/V2, PLAIN and dictionary encodings, flat optional columns,
+ * INT32 / INT64, Utf8View from BYTE_ARRAY).  INT32 also decodes to Int8, Int16, UInt8 and UInt16 (the INT(8|16, signed|unsigned)
+ * annotations): the value stored is the low bytes of the INT32, the truncation parquet-cpp and arrow-rs apply.  The library never
+ * sees a BYTE_ARRAY column's annotation, so which Arrow type it decodes to is the caller's choice: a UTF8-annotated column and a
+ * plain binary one both decode to Utf8View, bytes passed through unchanged and not validated as UTF-8.  A shim applying
+ * `binary_as_string` asks for Utf8View for the binary columns.  Covered: data pages V1/V2, PLAIN and dictionary encodings, flat optional columns,
  * uncompressed and ZSTD-compressed pages (codec 0 or 6; columns of both kinds may be mixed in one call); anything else, and
  * ZSTD frames that need a dictionary, returns SAILGPU_ERR_UNSUPPORTED and the caller keeps its CPU reader for that file.
  * ZSTD pages are decompressed on the device by one launch per call, covering every column; the decompressed chunk is read

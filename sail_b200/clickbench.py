@@ -29,6 +29,25 @@ def hits(columns):
     return scan("hits", columns)
 
 
+def view(columns: list) -> dict:
+    """The reference's view over hits.parquet (test_clickbench.py:134-136) as a projection spec over the stored `columns`
+    (datagen/hits.py:stored): EventDate, stored as UInt16 days since the epoch, becomes Date32 -- what
+    `date_add('1970-01-01', EventDate)` gives -- and every other column is passed through.  The binary strings are already
+    Utf8View when the scan reads them with `binary_as_string`; EventTime stays Int64 (see datagen/hits.py).  A projection
+    has at most 24 outputs, so the view is applied per scan, over the columns it reads (over_view), as DataFusion pushes the
+    view's projection into each scan."""
+    def expr(i, name):
+        return {"cast": {"col": i}, "to": "Date32"} if name == "EventDate" else {"col": i}
+    return {"op": "projection", "exprs": [{"expr": expr(i, n), "name": n} for i, n in enumerate(columns)]}
+
+
+def over_view(plan: Node) -> Node:
+    """`plan` with every scan of hits read through the view: the plan to run over the stored table (datagen/hits.py:stored)"""
+    if plan.spec["op"] == "scan":
+        return Node(view(plan.names), [plan], list(plan.names))
+    return Node(plan.spec, [over_view(c) for c in plan.inputs], list(plan.names))
+
+
 def ne_empty(c):
     return binop("!=", col(c), string(""))
 

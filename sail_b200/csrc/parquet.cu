@@ -8,9 +8,16 @@
 // headers of the RLE / bit-packed hybrid streams (a few bytes per run); every value is produced by a GPU thread.
 //
 // Covered: data pages V1 / V2, dictionary pages, PLAIN and RLE_DICTIONARY / PLAIN_DICTIONARY values, RLE definition
-// levels of flat optional columns (max level 1), physical types INT32 / INT64 / DOUBLE / FLOAT / FIXED_LEN_BYTE_ARRAY /
-// BYTE_ARRAY, uncompressed and ZSTD-compressed pages.  Other codecs, nested columns and the DELTA_* encodings are refused
-// (SAILGPU_ERR_UNSUPPORTED): the caller keeps the CPU reader for those files.
+// levels of flat optional columns (max level 1), physical types INT32 / INT64 / DOUBLE / FIXED_LEN_BYTE_ARRAY / BYTE_ARRAY,
+// uncompressed and ZSTD-compressed pages.  BOOLEAN, FLOAT and INT96 columns, other codecs, nested columns and the DELTA_*
+// encodings are refused (SAILGPU_ERR_UNSUPPORTED): the caller keeps the CPU reader for those files.
+//
+// INT32 decodes to Int32 / Date32, to Decimal128, and to the narrow integers Int8 / Int16 / UInt8 / UInt16 (how Parquet stores
+// the INT(8|16, signed|unsigned) logical types, e.g. ClickBench's Int16 columns and its UInt16 EventDate): the value kept is the
+// low 1 or 2 bytes of the INT32, which is how parquet-cpp and arrow-rs truncate.  BYTE_ARRAY decodes to Utf8View whatever the
+// column's annotation: the annotation never reaches this code, so a UTF8 string column and a plain binary one (ClickBench's URL,
+// Title, ... read with `binary_as_string`) take the same path.  The bytes are passed through unchanged and are not validated as
+// UTF-8; whether Sail's CPU reader rejects invalid UTF-8 in a binary column read as string is not checked here.
 //
 // ZSTD chunks (Sail's writer default) are decompressed on the device first.  Page headers are stored uncompressed, so the host
 // walks them into a page table (where each page's frames start, how long they are, where the decompressed body goes) and
@@ -197,7 +204,7 @@ struct DecodeParams {
   const Segment* segs; int n_segs;  // PLAIN pages
   const uint64_t* str_off;          // PLAIN BYTE_ARRAY: byte offset of every dense value's length prefix inside the chunk
   int64_t n_rows;
-  int physical, type_length, out_width;   // out_width: 4, 8, 16 (Decimal128) or 16 with is_view
+  int physical, type_length, out_width;   // out_width: 1 / 2 (narrow integers from INT32), 4, 8, 16 (Decimal128) or 16 with is_view
   int is_view;
   uint32_t dict_size;
   uint32_t* error;
@@ -225,7 +232,9 @@ __device__ __forceinline__ void store_plain(const DecodeParams& D, const uint8_t
     int32_t x; memcpy(&x, src, 4);
     if (D.out_width == 16) { ulonglong2 w; w.x = (unsigned long long)(long long)x; w.y = (unsigned long long)((long long)x >> 63); *reinterpret_cast<ulonglong2*>(dst) = w; }
     else if (D.out_width == 8) *reinterpret_cast<long long*>(dst) = x;
-    else *reinterpret_cast<int32_t*>(dst) = x;
+    else if (D.out_width == 4) *reinterpret_cast<int32_t*>(dst) = x;
+    else if (D.out_width == 2) *reinterpret_cast<uint16_t*>(dst) = (uint16_t)x;     // Int16 / UInt16: the low bytes of the INT32
+    else *dst = (uint8_t)x;                                                         // Int8 / UInt8
   } else {                                      // INT64 / DOUBLE
     long long x; memcpy(&x, src, 8);
     if (D.out_width == 16) { ulonglong2 w; w.x = (unsigned long long)x; w.y = (unsigned long long)(x >> 63); *reinterpret_cast<ulonglong2*>(dst) = w; }
@@ -239,7 +248,9 @@ __global__ void decode_values_kernel(DecodeParams D, uint8_t* __restrict__ out) 
     if (D.valid && !D.valid[i]) {
       if (D.out_width == 16) { ulonglong2 z; z.x = 0; z.y = 0; *reinterpret_cast<ulonglong2*>(dst) = z; }
       else if (D.out_width == 8) *reinterpret_cast<long long*>(dst) = 0;
-      else *reinterpret_cast<int32_t*>(dst) = 0;
+      else if (D.out_width == 4) *reinterpret_cast<int32_t*>(dst) = 0;
+      else if (D.out_width == 2) *reinterpret_cast<uint16_t*>(dst) = 0;
+      else *dst = 0;
       continue;
     }
     const int64_t v = D.vpos ? (int64_t)D.vpos[i] : i;
@@ -248,10 +259,12 @@ __global__ void decode_values_kernel(DecodeParams D, uint8_t* __restrict__ out) 
     if (D.segs[lo].is_dict) {
       const uint32_t k = D.dict_idx[v];
       if (k >= D.dict_size) { atomicOr(D.error, ERR_UNSUPPORTED); continue; }
-      const uint8_t* s = D.dict_vals + (size_t)k * D.out_width;
+      const uint8_t* s = D.dict_vals + (size_t)k * D.out_width;       // entries were decoded at the output width
       if (D.out_width == 16) *reinterpret_cast<ulonglong2*>(dst) = *reinterpret_cast<const ulonglong2*>(s);
       else if (D.out_width == 8) *reinterpret_cast<long long*>(dst) = *reinterpret_cast<const long long*>(s);
-      else *reinterpret_cast<int32_t*>(dst) = *reinterpret_cast<const int32_t*>(s);
+      else if (D.out_width == 4) *reinterpret_cast<int32_t*>(dst) = *reinterpret_cast<const int32_t*>(s);
+      else if (D.out_width == 2) *reinterpret_cast<uint16_t*>(dst) = *reinterpret_cast<const uint16_t*>(s);
+      else *dst = *s;
     } else if (D.is_view) {
       store_plain(D, D.chunk + D.str_off[v], dst);
     } else {
@@ -330,10 +343,11 @@ void check_parquet_column(const Field& f, const ParquetColumnDesc& c, int64_t n_
   SG_CHECK((pt == PT_BYTE_ARRAY) == is_str, SAILGPU_ERR_UNSUPPORTED, "parquet: BYTE_ARRAY columns decode to strings only (column '" + f.name + "')");
   SG_CHECK(f.type.id != TypeId::Utf8, SAILGPU_ERR_UNSUPPORTED, "parquet: strings decode to Utf8View (what Sail reads Parquet strings as: application.yaml:375-381)");
   const int out_width = is_str ? 16 : f.type.arrow_width();
-  SG_CHECK(out_width == 4 || out_width == 8 || out_width == 16, SAILGPU_ERR_UNSUPPORTED, "parquet: target type " + f.type.str());
+  const bool narrow = f.type.is_int() && out_width <= 2;                      // Int8 / Int16 / UInt8 / UInt16
+  SG_CHECK(narrow || out_width == 4 || out_width == 8 || out_width == 16, SAILGPU_ERR_UNSUPPORTED, "parquet: target type " + f.type.str());
   if (pt == PT_FLBA) SG_CHECK(f.type.is_decimal() && c.type_length >= 1 && c.type_length <= 16, SAILGPU_ERR_UNSUPPORTED, "parquet: FIXED_LEN_BYTE_ARRAY decodes to Decimal128 only");
   if (pt == PT_DOUBLE) SG_CHECK(f.type.id == TypeId::Float64, SAILGPU_ERR_UNSUPPORTED, "parquet: DOUBLE decodes to Float64");
-  if (pt == PT_INT32) SG_CHECK(out_width == 4 || f.type.is_decimal(), SAILGPU_ERR_UNSUPPORTED, "parquet: INT32 decodes to 32-bit types or Decimal128");
+  if (pt == PT_INT32) SG_CHECK(narrow || out_width == 4 || f.type.is_decimal(), SAILGPU_ERR_UNSUPPORTED, "parquet: INT32 decodes to 8-, 16- or 32-bit types or Decimal128");
   if (pt == PT_INT64) SG_CHECK(out_width == 8 || f.type.is_decimal(), SAILGPU_ERR_UNSUPPORTED, "parquet: INT64 decodes to 64-bit types or Decimal128");
 }
 

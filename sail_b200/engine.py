@@ -491,7 +491,7 @@ _PQ_PHYSICAL = {"BOOLEAN": 0, "INT32": 1, "INT64": 2, "INT96": 3, "FLOAT": 4, "D
 _PQ_CODEC = {"UNCOMPRESSED": 0, "SNAPPY": 1, "GZIP": 2, "LZO": 3, "BROTLI": 4, "LZ4": 5, "ZSTD": 6, "LZ4_RAW": 7}
 
 
-def _parquet_descriptors(file_bytes, row_group: int, columns: list | None):
+def _parquet_descriptors(file_bytes, row_group: int, columns: list | None, binary_as_string: bool = False):
     import pyarrow.parquet as pq
     buf = pa.py_buffer(file_bytes)
     f = pq.ParquetFile(pa.BufferReader(buf))
@@ -505,6 +505,8 @@ def _parquet_descriptors(file_bytes, row_group: int, columns: list | None):
         t = f.schema_arrow.field(name).type
         if pa.types.is_string(t) or pa.types.is_large_string(t):
             t = pa.string_view()
+        elif binary_as_string and (pa.types.is_binary(t) or pa.types.is_large_binary(t)):
+            t = pa.string_view()         # DataFusion's `binary_as_string`: unannotated BYTE_ARRAY columns read as strings
         fields.append(pa.field(name, t, nullable=cs.max_definition_level > 0))
         start = cm.data_page_offset
         if cm.has_dictionary_page and cm.dictionary_page_offset is not None:
@@ -520,11 +522,14 @@ def _parquet_descriptors(file_bytes, row_group: int, columns: list | None):
     return buf, pa.schema(fields), cols, rg.num_rows
 
 
-def parquet_decode(file_bytes, row_group: int = 0, columns: list | None = None, ctx: Context | None = None) -> DeviceBatch:
+def parquet_decode(file_bytes, row_group: int = 0, columns: list | None = None, ctx: Context | None = None,
+                   binary_as_string: bool = False) -> DeviceBatch:
     """One row group of a Parquet file (bytes in host memory) decoded on the device: the footer is read here with pyarrow (the
-    Rust side uses the `parquet` crate), the column chunks go to sailgpu_parquet_decode as stored."""
+    Rust side uses the `parquet` crate), the column chunks go to sailgpu_parquet_decode as stored.  binary_as_string: BYTE_ARRAY
+    columns without a UTF8 annotation decode to Utf8View (their bytes unchanged, not validated as UTF-8); without it such a
+    column is refused (SAILGPU_ERR_UNSUPPORTED), as the library has no binary type."""
     ctx = ctx or default_context()
-    buf, schema, cols, n_rows = _parquet_descriptors(file_bytes, row_group, columns)
+    buf, schema, cols, n_rows = _parquet_descriptors(file_bytes, row_group, columns, binary_as_string)
     cschema = _export_schema(schema)
     d = DeviceBatch(schema)
     rc = lib().sailgpu_parquet_decode(ctx._h, ctypes.addressof(cschema), ctypes.addressof(cols), len(cols), n_rows, ctypes.addressof(d.c))
@@ -536,9 +541,9 @@ def parquet_decode(file_bytes, row_group: int = 0, columns: list | None = None, 
     return d
 
 
-def parquet_inspect(file_bytes, column: int, row_group: int = 0, columns: list | None = None) -> dict:
+def parquet_inspect(file_bytes, column: int, row_group: int = 0, columns: list | None = None, binary_as_string: bool = False) -> dict:
     """Host-only: what the page / run-header walk of sailgpu_parquet_decode finds in one column chunk (no GPU needed)."""
-    buf, schema, cols, n_rows = _parquet_descriptors(file_bytes, row_group, columns)
+    buf, schema, cols, n_rows = _parquet_descriptors(file_bytes, row_group, columns, binary_as_string)
     cschema = _export_schema(schema)
     out = ctypes.create_string_buffer(1024)
     rc = lib().sailgpu_parquet_inspect(ctypes.addressof(cschema), ctypes.addressof(cols), len(cols), n_rows, column, out, 1024)
