@@ -59,9 +59,19 @@
  * Expressions E: {"col":i} {"lit":v,"type":"T"} {"op":"+|-|*|/|%|=|!=|<|<=|>|>=|and|or","l":E,"r":E}
  *   {"not":E} {"neg":E} {"is_null":E} {"is_not_null":E} {"cast":E,"to":"T"}
  *   {"case":[[E,E],...],"else":E|null} {"in":E,"set":[lit,...],"negated":b}
- *   {"like":E,"pattern":"..","negated":b} {"fn":"date_part","part":"year|month|day","args":[E]}
+ *   {"like":E,"pattern":"..","negated":b} {"fn":"date_part","part":"year|month|day","args":[E]}   (E Date32)
+ *   {"fn":"date_part","part":"year|quarter|month|day|hour|minute|second","args":[E]}   (E Timestamp: Int32, second as
+ *                                           Decimal128(8,6), the microsecond within the minute; in the column's zone)
+ *   {"fn":"date_trunc","part":"year|quarter|month|week|day|hour|minute|second","args":[E]}   (E Timestamp -> its type)
  *   {"fn":"substr","args":[E],"start":s,"length":n|null}   (1-based, in characters)
  * Types T: Boolean Int8..Int64 UInt8..UInt64 Float32 Float64 Date32 Decimal128(p,s) Utf8 Utf8View
+ *   Timestamp(s|ms|us|ns[, zone]) (Arrow tss: / tsm: / tsu: / tsn: + zone; stored as Int64).  Any zone passes through the
+ *   operators; date_part, date_trunc and the cast to Date32 read wall-clock time and accept no zone, UTC or +HH:MM / -HH:MM
+ *   only (other zones: SAILGPU_ERR_UNSUPPORTED).  Casts: Int64 <-> Timestamp (same value), Timestamp -> Date32, Timestamp ->
+ *   Timestamp of the same or a finer unit; comparisons between timestamps of one unit; no arithmetic, sum or avg.
+ *   Range: the calendar parts and truncations (year .. day, week) and the cast to Date32 count days in 32 bits, so they are exact
+ *   for instants within about 5.8 million years of the epoch (Date32's range) and wrong beyond it, which only Timestamp(s) and
+ *   Timestamp(ms) can reach; the cast to a finer unit wraps when the product leaves int64 (arrow-rs reports an error there).
  *
  * Threading (SURVEY.md section 8b): any function may be called from any thread (no affinity: the
  * device is set per call); calls on one handle must not overlap.  A context owns ONE compute stream,
@@ -189,7 +199,9 @@ SAILGPU_API int32_t sailgpu_spec_validate(const char* spec_json, size_t spec_len
  * exactly as stored in the file (dictionary page first) plus what the footer says about it; the chunk crosses PCIe as stored and is
  * decoded on the device (page headers and RLE run headers are walked on the host, every value is produced by a GPU thread).
  * `schema` names the Arrow type each column decodes to (Int32/Date32, Int64, Float64, Decimal128 from FIXED_LEN_BYTE_ARRAY /
- * INT32 / INT64, Utf8View from BYTE_ARRAY).  INT32 also decodes to Int8, Int16, UInt8 and UInt16 (the INT(8|16, signed|unsigned)
+ * INT32 / INT64, Utf8View from BYTE_ARRAY, Timestamp from INT64 annotated TIMESTAMP(MILLIS|MICROS|NANOS, isAdjustedToUTC): the
+ * annotation never reaches the library, the caller names the unit and zone and the 8-byte values pass through unchanged; INT96
+ * stays refused).  INT32 also decodes to Int8, Int16, UInt8 and UInt16 (the INT(8|16, signed|unsigned)
  * annotations): the value stored is the low bytes of the INT32, the truncation parquet-cpp and arrow-rs apply.  The library never
  * sees a BYTE_ARRAY column's annotation, so which Arrow type it decodes to is the caller's choice: a UTF8-annotated column and a
  * plain binary one both decode to Utf8View, bytes passed through unchanged and not validated as UTF-8.  A shim applying

@@ -26,14 +26,26 @@ struct Error : std::runtime_error {
 // ------------------------------------------------------------------------------------------------
 enum class TypeId : uint8_t {
   Bool, Int8, Int16, Int32, Int64, UInt8, UInt16, UInt32, UInt64, Float32, Float64, Date32,
-  Decimal128, Utf8, Utf8View, Null
+  Decimal128, Utf8, Utf8View, Timestamp, Null
 };
+
+enum TimeUnit : int { TU_S = 0, TU_MS = 1, TU_US = 2, TU_NS = 3 };
+inline int64_t unit_per_second(int unit) { return unit == TU_S ? 1 : unit == TU_MS ? 1000 : unit == TU_US ? 1000000 : 1000000000; }
 
 struct DataType {
   TypeId id = TypeId::Null;
   int precision = 0, scale = 0;
-  bool operator==(const DataType& o) const { return id == o.id && precision == o.precision && scale == o.scale; }
+  int unit = TU_S;        // Timestamp: TimeUnit
+  std::string tz;         // Timestamp: zone as Arrow carries it ("" = none)
+  bool operator==(const DataType& o) const {
+    return id == o.id && precision == o.precision && scale == o.scale && unit == o.unit && tz == o.tz;
+  }
   bool operator!=(const DataType& o) const { return !(*this == o); }
+  bool is_timestamp() const { return id == TypeId::Timestamp; }
+  // How values are laid out and compared on the device.  A Timestamp is stored as Int64 (Arrow's layout); everything that
+  // moves, hashes, compares or accumulates values asks for this type, so only expressions that read wall-clock time know
+  // the Timestamp type itself.
+  DataType storage() const;
   bool is_decimal() const { return id == TypeId::Decimal128; }
   bool is_string() const { return id == TypeId::Utf8 || id == TypeId::Utf8View; }
   bool is_float() const { return id == TypeId::Float32 || id == TypeId::Float64; }
@@ -47,7 +59,7 @@ struct DataType {
       case TypeId::Int8: case TypeId::UInt8: return 1;
       case TypeId::Int16: case TypeId::UInt16: return 2;
       case TypeId::Int32: case TypeId::UInt32: case TypeId::Float32: case TypeId::Date32: return 4;
-      case TypeId::Int64: case TypeId::UInt64: case TypeId::Float64: return 8;
+      case TypeId::Int64: case TypeId::UInt64: case TypeId::Float64: case TypeId::Timestamp: return 8;
       case TypeId::Decimal128: case TypeId::Utf8View: return 16;
       case TypeId::Utf8: return 4;
       default: return 0;
@@ -59,6 +71,24 @@ struct DataType {
 
 inline DataType T(TypeId id) { DataType t; t.id = id; return t; }
 inline DataType Dec(int p, int s) { DataType t; t.id = TypeId::Decimal128; t.precision = p; t.scale = s; return t; }
+inline DataType Ts(int unit, const std::string& tz) { DataType t; t.id = TypeId::Timestamp; t.unit = unit; t.tz = tz; return t; }
+inline DataType DataType::storage() const { return id == TypeId::Timestamp ? T(TypeId::Int64) : *this; }
+
+inline const char* unit_name(int unit) { return unit == TU_S ? "s" : unit == TU_MS ? "ms" : unit == TU_US ? "us" : "ns"; }
+
+// Zone of a Timestamp as the functions that read wall-clock time need it: the offset from UTC in seconds.  Accepted: no zone,
+// "UTC", and fixed offsets "+HH:MM" / "-HH:MM".  Anything else (an IANA name such as "Europe/Paris") needs a time-zone
+// database and is refused.
+inline int64_t zone_offset_seconds(const std::string& tz) {
+  if (tz.empty() || tz == "UTC") return 0;
+  int hh = 0, mm = 0;
+  char sign = 0, colon = 0;
+  if (tz.size() == 6 && sscanf(tz.c_str(), "%c%2d%c%2d", &sign, &hh, &colon, &mm) == 4 && (sign == '+' || sign == '-') && colon == ':' &&
+      isdigit((unsigned char)tz[1]) && isdigit((unsigned char)tz[2]) && isdigit((unsigned char)tz[4]) && isdigit((unsigned char)tz[5]) &&
+      hh <= 23 && mm <= 59)
+    return (sign == '-' ? -1 : 1) * (int64_t)(hh * 3600 + mm * 60);
+  fail(SAILGPU_ERR_UNSUPPORTED, "time zone '" + tz + "' is not supported on the GPU path (only UTC and fixed offsets +HH:MM)");
+}
 
 inline std::string DataType::str() const {
   switch (id) {
@@ -71,6 +101,7 @@ inline std::string DataType::str() const {
     case TypeId::Date32: return "Date32";
     case TypeId::Decimal128: return "Decimal128(" + std::to_string(precision) + "," + std::to_string(scale) + ")";
     case TypeId::Utf8: return "Utf8"; case TypeId::Utf8View: return "Utf8View";
+    case TypeId::Timestamp: return std::string("Timestamp(") + unit_name(unit) + (tz.empty() ? "" : ", " + tz) + ")";
     default: return "Null";
   }
 }
@@ -85,6 +116,7 @@ inline std::string DataType::arrow_format() const {
     case TypeId::Date32: return "tdD";
     case TypeId::Decimal128: return "d:" + std::to_string(precision) + "," + std::to_string(scale);
     case TypeId::Utf8: return "u"; case TypeId::Utf8View: return "vu";
+    case TypeId::Timestamp: return std::string("ts") + "smun"[unit] + ":" + tz;
     default: return "n";
   }
 }
@@ -99,6 +131,17 @@ inline DataType parse_type(const std::string& s) {
   int p = 0, sc = 0;
   if (sscanf(s.c_str(), "Decimal128(%d,%d)", &p, &sc) == 2 || sscanf(s.c_str(), "Decimal128(%d, %d)", &p, &sc) == 2)
     return Dec(p, sc);
+  if (s.size() > 11 && s.compare(0, 10, "Timestamp(") == 0 && s.back() == ')') {   // Timestamp(<unit>[, <zone>])
+    std::string body = s.substr(10, s.size() - 11), u = body, tz;
+    const size_t comma = body.find(',');
+    if (comma != std::string::npos) {
+      u = body.substr(0, comma);
+      tz = body.substr(comma + 1);
+      while (!tz.empty() && tz.front() == ' ') tz.erase(0, 1);
+    }
+    for (int k = TU_S; k <= TU_NS; ++k)
+      if (u == unit_name(k)) return Ts(k, tz);
+  }
   fail(SAILGPU_ERR_UNSUPPORTED, "unsupported data type '" + s + "'");
 }
 inline DataType type_from_arrow_format(const char* f) {
@@ -111,6 +154,11 @@ inline DataType type_from_arrow_format(const char* f) {
   if (s == "f") return T(TypeId::Float32); if (s == "g") return T(TypeId::Float64);
   if (s == "tdD") return T(TypeId::Date32);
   if (s == "u") return T(TypeId::Utf8); if (s == "vu") return T(TypeId::Utf8View);
+  if (s.size() >= 4 && s[0] == 't' && s[1] == 's' && s[3] == ':') {   // tss: / tsm: / tsu: / tsn: followed by the zone (may be empty)
+    const char* units = "smun";
+    const char* u = strchr(units, s[2]);
+    if (s[2] && u) return Ts((int)(u - units), s.substr(4));
+  }
   int p = 0, sc = 0, bits = 128;
   if (sscanf(f, "d:%d,%d,%d", &p, &sc, &bits) >= 2) {
     SG_CHECK(bits == 128, SAILGPU_ERR_UNSUPPORTED, "only 128-bit decimals are supported");

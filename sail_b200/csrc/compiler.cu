@@ -11,7 +11,7 @@ static uint64_t lo64(i128 v) { return (uint64_t)(u128)v; }
 static uint64_t hi64(i128 v) { return (uint64_t)((u128)v >> 64); }
 
 Val PipelineCompiler::input_value(int col) {
-  const DataType& t = in_[(size_t)col].type;
+  const DataType t = in_[(size_t)col].type.storage();
   auto reg = [&](bool validity, uint16_t width) {
     auto key = std::make_pair(col, validity);
     auto it = input_slot_.find(key);
@@ -159,6 +159,15 @@ Val PipelineCompiler::compile_cast(const ExprPtr& e) {
   const int K = phys_kind(to);
   Val d;
   if (from.is_string() && to.is_string()) return v;
+  if (from.is_timestamp() || to.is_timestamp()) {
+    // expr.hpp: make_cast admits only these; anything else reaching here is refused rather than relabelled
+    if (from.is_timestamp() && to.id == TypeId::Date32) return ts_op(OP_TS_PART, K_I32, TS_DAYS, v, from);
+    if (from.is_timestamp() && to.is_timestamp() && to.unit >= from.unit) d = mul_pow10(v, 3 * (to.unit - from.unit));
+    else if ((from.is_timestamp() && to.id == TypeId::Int64) || (from.id == TypeId::Int64 && to.is_timestamp())) d = v;   // same value
+    else fail(SAILGPU_ERR_UNSUPPORTED, "cast " + from.str() + " -> " + to.str());
+    d.vslot = v.vslot;
+    return d;
+  }
   if (to.is_decimal()) {
     if (from.is_decimal()) {
       if (to.scale >= from.scale) d = mul_pow10(convert(v, K), to.scale - from.scale);
@@ -183,6 +192,15 @@ Val PipelineCompiler::compile_cast(const ExprPtr& e) {
     d = v;
   } else fail(SAILGPU_ERR_UNSUPPORTED, "cast " + from.str() + " -> " + to.str());
   d.vslot = v.vslot;
+  return d;
+}
+
+Val PipelineCompiler::ts_op(int base, int dst_kind, int part, const Val& a, const DataType& t) {
+  const int64_t ups = unit_per_second(t.unit);
+  Val d = emit1(base, dst_kind, dst_kind, a, (uint16_t)part);
+  prog_.back().imm0 = (uint64_t)ups;
+  prog_.back().imm1 = (uint64_t)(zone_offset_seconds(t.tz) * ups);
+  d.vslot = a.vslot;
   return d;
 }
 
@@ -267,7 +285,15 @@ Val PipelineCompiler::compile_uncached(const ExprPtr& e) {
       out.vslot = a.vslot;
       return out;
     }
+    case Expr::DateTrunc: {
+      const DataType& t = e->args[0]->type;
+      return ts_op(OP_TS_TRUNC, K_I64, timestamp_part("date_trunc", e->op), compile(e->args[0]), t);
+    }
     case Expr::DatePart: {
+      if (e->args[0]->type.is_timestamp()) {
+        const int part = timestamp_part("date_part", e->op);
+        return ts_op(OP_TS_PART, part == TS_SECOND ? K_I64 : K_I32, part, compile(e->args[0]), e->args[0]->type);
+      }
       Val a = compile(e->args[0]);
       Val d = emit1(OP_DATE_PART, K_I32, K_I32, a, (uint16_t)(e->op == "year" ? 0 : e->op == "month" ? 1 : 2));
       d.vslot = a.vslot;

@@ -223,7 +223,8 @@ class PipelineCompiler {
   std::vector<DataType> out_types_;
   std::vector<int> out_kinds_;
 
-  static int phys_kind(const DataType& t) {
+  static int phys_kind(const DataType& type) {
+    const DataType t = type.storage();
     switch (t.id) {
       case TypeId::Bool: return K_B;
       case TypeId::Int8: case TypeId::Int16: case TypeId::Int32: case TypeId::UInt8: case TypeId::UInt16: case TypeId::Date32: return K_I32;
@@ -354,6 +355,8 @@ class PipelineCompiler {
   }
   Val compile_bin(const ExprPtr& e);
   Val compile_cast(const ExprPtr& e);
+  // OP_TS_PART / OP_TS_TRUNC over timestamp value `a` of type `t`: unit and zone offset travel in the immediates
+  Val ts_op(int base, int dst_kind, int part, const Val& a, const DataType& t);
   Val compile_uncached(const ExprPtr& e);
 };
 

@@ -40,6 +40,66 @@ __device__ __forceinline__ void civil_from_days(int32_t z0, int& y, int& m, int&
   m = (int)(mp < 10 ? mp + 3 : mp - 9);
   y = (int)(m <= 2 ? yy + 1 : yy);
 }
+// civil (year, month, day) -> days since 1970-01-01: the inverse of civil_from_days
+__device__ __forceinline__ int32_t days_from_civil(int y, int m, int d) {
+  y -= m <= 2;
+  const int era = (y >= 0 ? y : y - 399) / 400;
+  const int yoe = y - era * 400;
+  const int doy = (153 * (m > 2 ? m - 3 : m + 9) + 2) / 5 + d - 1;
+  const int doe = yoe * 365 + yoe / 4 - yoe / 100 + doy;
+  return era * 146097 + doe - 719468;
+}
+
+// ---- timestamps (Int64 counts of UPS units per second since the epoch) --------------------------------------------------
+// OP_TS_PART / OP_TS_TRUNC read wall-clock time in a fixed-offset zone: `off` is the offset from UTC in units.  The unit is a
+// template argument, so every division below is by a compile-time constant and becomes a multiply-high: the interpreter
+// dispatches once per instruction on the unit (pipeline.cu: vm_ts), the specialised kernel names it in the generated code.
+// The calendar parts go through 32-bit day counts: exact within Date32's range (about 5.8 million years around the epoch).
+template <int64_t D> __device__ __forceinline__ int64_t floor_div_c(int64_t a) {
+  const int64_t q = a / D;
+  return a - q * D < 0 ? q - 1 : q;
+}
+template <int64_t UPS> __device__ __forceinline__ int64_t ts_part_u(int64_t v, int part, int64_t off) {
+  constexpr int64_t DAY = 86400 * UPS;
+  const int64_t local = (int64_t)((uint64_t)v + (uint64_t)off);
+  const int64_t days = floor_div_c<DAY>(local);
+  const int64_t tod = local - days * DAY;      // [0, DAY)
+  switch (part) {
+    case TS_HOUR: return tod / (3600 * UPS);
+    case TS_MINUTE: return (tod / (60 * UPS)) % 60;
+    case TS_SECOND: {                           // microsecond within the minute (the unscaled Decimal128(8,6) of Spark's second)
+      const int64_t r = tod % (60 * UPS);
+      if constexpr (UPS <= 1000000) return r * (1000000 / UPS);
+      else return r / (UPS / 1000000);
+    }
+    case TS_DAYS: return days;
+    default: break;
+  }
+  int y, m, d;
+  civil_from_days((int32_t)days, y, m, d);
+  return part == TS_YEAR ? y : part == TS_QUARTER ? (m - 1) / 3 + 1 : part == TS_MONTH ? m : d;
+}
+template <int64_t UPS> __device__ __forceinline__ int64_t ts_trunc_u(int64_t v, int part, int64_t off) {
+  constexpr int64_t DAY = 86400 * UPS;
+  const int64_t local = (int64_t)((uint64_t)v + (uint64_t)off);
+  const int64_t days = floor_div_c<DAY>(local);
+  const int64_t tod = local - days * DAY;
+  int64_t t;
+  switch (part) {
+    case TS_SECOND: t = local - tod % UPS; break;
+    case TS_MINUTE: t = local - tod % (60 * UPS); break;
+    case TS_HOUR: t = local - tod % (3600 * UPS); break;
+    case TS_DAY: t = days * DAY; break;
+    case TS_WEEK: t = (days - (days + 3 - floor_div_c<7>(days + 3) * 7)) * DAY; break;    // ISO weeks start on Monday; 1970-01-01 was a Thursday
+    default: {
+      int y, m, d;
+      civil_from_days((int32_t)days, y, m, d);
+      m = part == TS_YEAR ? 1 : part == TS_QUARTER ? (m - 1) / 3 * 3 + 1 : m;
+      t = (int64_t)days_from_civil(y, m, 1) * DAY;
+    }
+  }
+  return (int64_t)((uint64_t)t - (uint64_t)off);
+}
 
 __device__ __forceinline__ bool like_match(const uint8_t* s, uint32_t n, const uint8_t* p, uint32_t m, int cls) {
   switch (cls) {

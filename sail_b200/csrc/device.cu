@@ -214,7 +214,7 @@ DevColumn import_column(ImportJob& J, const Field& f, const ArrowArray* a, const
       const uint8_t* p = static_cast<const uint8_t*>(a->buffers[1]) + a->offset * w;
       if (on_device) c.data = borrow(p, (size_t)a->length * w);
       else {
-        const TypeId id = f.type.id;
+        const TypeId id = f.type.storage().id;
         const HostCol kind = id == TypeId::Decimal128 ? HostCol::Dec128
                            : (id == TypeId::Int64 || id == TypeId::UInt64) ? HostCol::Int64
                            : (id == TypeId::Int32 || id == TypeId::UInt32 || id == TypeId::Date32) ? HostCol::Int32 : HostCol::Raw;

@@ -8,6 +8,7 @@
 #include <algorithm>
 
 #include "common.hpp"
+#include "vm.h"
 
 namespace sg {
 
@@ -15,7 +16,7 @@ struct Expr;
 using ExprPtr = std::shared_ptr<Expr>;
 
 struct Expr {
-  enum Kind { Col, Lit, Bin, Not, Neg, IsNull, IsNotNull, Cast, Case, Like, DatePart, Substr } kind = Col;
+  enum Kind { Col, Lit, Bin, Not, Neg, IsNull, IsNotNull, Cast, Case, Like, DatePart, Substr, DateTrunc } kind = Col;
   DataType type;
   bool nullable = false;
   // Col
@@ -74,11 +75,38 @@ inline DataType decimal_result(const std::string& op, const DataType& a, const D
   fail(SAILGPU_ERR_INVALID, "bad decimal op " + op);
 }
 
+// Casts that involve a Timestamp (arrow-rs semantics): Int64 <-> Timestamp reinterpret the value, Timestamp -> Date32 takes the
+// local date in the column's zone, Timestamp -> Timestamp of the same or a finer unit multiplies.  Everything else is refused.
+inline void check_timestamp_cast(const DataType& from, const DataType& to) {
+  if (!from.is_timestamp() && !to.is_timestamp()) return;
+  const std::string what = "cast " + from.str() + " -> " + to.str();
+  if (from.is_timestamp() && to.is_timestamp()) {
+    SG_CHECK(to.unit >= from.unit, SAILGPU_ERR_UNSUPPORTED, what + " (to a coarser unit) is not supported on the GPU path");
+    // between two zones the instant is kept; adding or dropping a zone would reinterpret wall-clock time
+    SG_CHECK(from.tz == to.tz || (!from.tz.empty() && !to.tz.empty()), SAILGPU_ERR_UNSUPPORTED, what + " is not supported on the GPU path");
+    return;
+  }
+  if (from.is_timestamp() && to.id == TypeId::Date32) { zone_offset_seconds(from.tz); return; }
+  SG_CHECK((from.is_timestamp() && to.id == TypeId::Int64) || (to.is_timestamp() && from.id == TypeId::Int64), SAILGPU_ERR_UNSUPPORTED,
+           what + " is not supported on the GPU path");
+}
+
+// Every cast, explicit or implied (CASE branches brought to one type, operand coercion), is built here, so the Timestamp
+// rules hold for all of them.
 inline ExprPtr make_cast(ExprPtr e, const DataType& to) {
   if (e->type == to) return e;
+  check_timestamp_cast(e->type, to);
   auto c = std::make_shared<Expr>();
   c->kind = Expr::Cast; c->type = to; c->nullable = e->nullable; c->args = {e};
   return c;
+}
+
+// date_part / date_trunc parts on a Timestamp (vm.h: TsPart); -1 = not a part of `fn`
+inline int timestamp_part(const std::string& fn, const std::string& part) {
+  static const char* names[] = {"year", "quarter", "month", "week", "day", "hour", "minute", "second"};
+  for (int k = TS_YEAR; k <= TS_SECOND; ++k)
+    if (part == names[k]) return fn == "date_part" && k == TS_WEEK ? -1 : k;
+  return -1;
 }
 
 inline bool is_arith(const std::string& op) { return op == "+" || op == "-" || op == "*" || op == "/" || op == "%"; }
@@ -128,7 +156,11 @@ inline ExprPtr make_bin(const std::string& op, ExprPtr l, ExprPtr r) {
       e->type = l->type;
     }
   } else if (is_cmp(op)) {
-    if (l->type.is_string() && r->type.is_string()) {
+    if (l->type.is_timestamp() || r->type.is_timestamp()) {
+      // instants compare across zones; across units they would need a rescale, which DataFusion's coercion adds as a cast
+      SG_CHECK(l->type.is_timestamp() && r->type.is_timestamp() && l->type.unit == r->type.unit, SAILGPU_ERR_UNSUPPORTED,
+               "comparison of " + l->type.str() + " and " + r->type.str());
+    } else if (l->type.is_string() && r->type.is_string()) {
       SG_CHECK(op == "=" || op == "!=", SAILGPU_ERR_UNSUPPORTED, "ordering comparison on strings is not supported on the GPU path yet");
     } else {
       coerce_numeric(l, r, true);
@@ -165,6 +197,7 @@ inline ExprPtr parse_expr(const Json& j, const Schema& in) {
   }
   if (j.has("neg")) {
     e->kind = Expr::Neg; e->args = {parse_expr(j.at("neg"), in)}; e->type = e->args[0]->type; e->nullable = e->args[0]->nullable;
+    SG_CHECK(!e->type.is_timestamp(), SAILGPU_ERR_UNSUPPORTED, "negation of " + e->type.str());
     return e;
   }
   if (j.has("is_null") || j.has("is_not_null")) {
@@ -225,13 +258,25 @@ inline ExprPtr parse_expr(const Json& j, const Schema& in) {
   }
   if (j.has("fn")) {
     const std::string fn = j.at("fn").as_str();
-    if (fn == "date_part") {
-      e->kind = Expr::DatePart; e->op = j.at("part").as_str();
-      std::transform(e->op.begin(), e->op.end(), e->op.begin(), ::tolower);
-      SG_CHECK(e->op == "year" || e->op == "month" || e->op == "day", SAILGPU_ERR_UNSUPPORTED, "date_part('" + e->op + "')");
-      e->args = {parse_expr(j.at("args").a.at(0), in)};
-      SG_CHECK(e->args[0]->type.id == TypeId::Date32, SAILGPU_ERR_UNSUPPORTED, "date_part on " + e->args[0]->type.str());
-      e->type = T(TypeId::Int32); e->nullable = e->args[0]->nullable;
+    if (fn == "date_part" || fn == "date_trunc") {
+      // On a Timestamp: the part in the column's zone (date_part: Int32, second as Decimal128(8,6) like Spark's; date_trunc: the
+      // input's type).  On a Date32: date_part of year, month or day, as Int32.
+      ExprPtr x = parse_expr(j.at("args").a.at(0), in);
+      std::string part = j.at("part").as_str();
+      std::transform(part.begin(), part.end(), part.begin(), ::tolower);
+      e->op = part; e->args = {x}; e->nullable = x->nullable;
+      if (x->type.is_timestamp()) {
+        const int k = timestamp_part(fn, part);
+        SG_CHECK(k >= 0, SAILGPU_ERR_UNSUPPORTED, fn + "('" + part + "') on " + x->type.str());
+        zone_offset_seconds(x->type.tz);
+        e->kind = fn == "date_part" ? Expr::DatePart : Expr::DateTrunc;
+        e->type = fn == "date_trunc" ? x->type : k == TS_SECOND ? Dec(8, 6) : T(TypeId::Int32);
+        return e;
+      }
+      SG_CHECK(fn == "date_part", SAILGPU_ERR_UNSUPPORTED, "date_trunc on " + x->type.str());
+      SG_CHECK(part == "year" || part == "month" || part == "day", SAILGPU_ERR_UNSUPPORTED, "date_part('" + part + "')");
+      SG_CHECK(x->type.id == TypeId::Date32, SAILGPU_ERR_UNSUPPORTED, "date_part on " + x->type.str());
+      e->kind = Expr::DatePart; e->type = T(TypeId::Int32);
       return e;
     }
     if (fn == "substr") {      // substr(str, start[, length]) with literal positions (Spark / DataFusion character semantics)
@@ -258,6 +303,7 @@ inline AggTypes agg_types(const std::string& fn, const DataType& in) {
   AggTypes t;
   if (fn == "count") { t.state = {T(TypeId::Int64)}; t.final_type = T(TypeId::Int64); return t; }
   if (fn == "min" || fn == "max") { t.state = {in}; t.final_type = in; return t; }
+  SG_CHECK(!in.is_timestamp(), SAILGPU_ERR_UNSUPPORTED, fn + " over " + in.str());
   if (fn == "sum") {
     DataType s = in.is_decimal() ? Dec(std::min(38, in.precision + 10), in.scale)
                : in.is_float() ? T(TypeId::Float64) : in.is_unsigned_int() ? T(TypeId::UInt64) : T(TypeId::Int64);

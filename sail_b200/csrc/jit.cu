@@ -218,6 +218,12 @@ struct Emitter {
         break;
       }
       case OP_DATE_PART: def(I.dst, K_I32, "jit_date_part(" + operand(I.a, K_I32, I.sa) + ", " + std::to_string(I.aux) + ")"); break;
+      case OP_TS_PART: case OP_TS_TRUNC: {   // unit and zone offset become constants: the divisions strength-reduce
+        const std::string call = std::string(base == OP_TS_TRUNC ? "ts_trunc_u<" : "ts_part_u<") + std::to_string((long long)I.imm0) + "ll>(" +
+                                 operand(I.a, K_I64, I.sa) + ", " + std::to_string(I.aux) + ", " + std::to_string((long long)I.imm1) + "ll)";
+        def(I.dst, kind, kind == K_I32 ? "(int32_t)" + call : call);
+        break;
+      }
       default: throw Unsupported{"VM instruction " + std::to_string(base)};
     }
   }

@@ -126,7 +126,7 @@ struct JoinOp : Op {
   // gathered build column `b` as a VM value (validity: gathered bytes AND `outer_valid` when given)
   Val gather_col(PipelineCompiler& pc, const Val& row, int b, const Val* outer_valid) {
     const DevColumn& c = build->cols[(size_t)b];
-    const DataType& t = bs[(size_t)b].type;
+    const DataType t = bs[(size_t)b].type.storage();
     int idx = -1;
     Val v;
     auto set_ptr = [&](const void* p) { pc.prog()[(size_t)idx].imm1 = reinterpret_cast<uint64_t>(p); };
@@ -886,7 +886,7 @@ struct SortOp : Op {
     for (size_t k = 0; k < ks.size(); ++k) {
       SG_CHECK(ks[k].e->kind == Expr::Col, SAILGPU_ERR_UNSUPPORTED, "sort keys must be column references");
       const DevColumn& c = all->cols[(size_t)ks[k].e->col];
-      const DataType& t = sch[(size_t)ks[k].e->col].type;
+      const DataType t = sch[(size_t)ks[k].e->col].type.storage();
       SortKeyCol& s = E.cols[k];
       s.data = static_cast<const uint8_t*>(c.data->ptr);
       s.validity_bits = c.validity ? static_cast<const uint8_t*>(c.validity->ptr) : nullptr;

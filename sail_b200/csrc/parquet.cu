@@ -17,7 +17,9 @@
 // low 1 or 2 bytes of the INT32, which is how parquet-cpp and arrow-rs truncate.  BYTE_ARRAY decodes to Utf8View whatever the
 // column's annotation: the annotation never reaches this code, so a UTF8 string column and a plain binary one (ClickBench's URL,
 // Title, ... read with `binary_as_string`) take the same path.  The bytes are passed through unchanged and are not validated as
-// UTF-8; whether Sail's CPU reader rejects invalid UTF-8 in a binary column read as string is not checked here.
+// UTF-8; whether Sail's CPU reader rejects invalid UTF-8 in a binary column read as string is not checked here.  INT64 columns
+// annotated TIMESTAMP(MILLIS|MICROS|NANOS, isAdjustedToUTC) decode to the Timestamp type the caller names, in the same way: the
+// annotation does not reach this code, and the 8-byte values pass through unchanged.  INT96 timestamps stay refused.
 //
 // ZSTD chunks (Sail's writer default) are decompressed on the device first.  Page headers are stored uncompressed, so the host
 // walks them into a page table (where each page's frames start, how long they are, where the decompressed body goes) and

@@ -273,6 +273,33 @@ __device__ __noinline__ void vm_like(const VmInst& I, const TileCtx& c) {
   }
 }
 
+// OP_TS_PART / OP_TS_TRUNC: out of line, so that the main VM switch keeps its registers.  The unit is chosen once per
+// instruction, outside the row loop, so each loop divides by constants only.
+template <int RPT, int64_t UPS, bool TRUNC>
+__device__ __forceinline__ void vm_ts_rows(const VmInst& I, const TileCtx& c) {
+  const uint8_t* pa = c.arena + eff(c, I.a);
+  uint8_t* pd = c.arena + eff(c, I.dst);
+  const int part = I.aux, kind = I.op >> 8;
+  const int64_t off = (int64_t)I.imm1;
+#pragma unroll
+  for (int k = 0; k < RPT; ++k) {
+    const int r = threadIdx.x + k * NT;
+    const int64_t v = lds<int64_t>(pa + r * I.sa);
+    const int64_t x = TRUNC ? ts_trunc_u<UPS>(v, part, off) : ts_part_u<UPS>(v, part, off);
+    if (kind == K_I32) sts<int32_t>(pd + r * 4, (int32_t)x);
+    else sts<int64_t>(pd + r * 8, x);
+  }
+}
+template <int RPT, bool TRUNC>
+__device__ __noinline__ void vm_ts(const VmInst& I, const TileCtx& c) {
+  switch (I.imm0) {
+    case 1: vm_ts_rows<RPT, 1, TRUNC>(I, c); break;
+    case 1000: vm_ts_rows<RPT, 1000, TRUNC>(I, c); break;
+    case 1000000: vm_ts_rows<RPT, 1000000, TRUNC>(I, c); break;
+    default: vm_ts_rows<RPT, 1000000000, TRUNC>(I, c);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // join probe (OP_PROBE): open-addressing lookup of the probe key in the build table
 // ------------------------------------------------------------------------------------------------
@@ -644,6 +671,8 @@ __device__ __forceinline__ void vm_exec(const VmInst* prog, int n_inst, const Ti
         }
         break;
       }
+      case OP_TS_PART: vm_ts<RPT, false>(I, c); break;
+      case OP_TS_TRUNC: vm_ts<RPT, true>(I, c); break;
       case OP_PROBE: vm_probe<RPT>(aux->probe[I.aux], c, I.c); break;
       case OP_GATHER: vm_gather<RPT>(I, c); break;
       default: break;

@@ -52,8 +52,14 @@ enum VmBase : uint16_t {
   OP_PROBE,         // hash-join probe: aux = probe index (see ProbeParams)
   OP_GATHER,        // dst(kind) <- build column [imm1 ptr] at row id slot a (I64), masked by active; aux = elem width
   OP_SUBSTR,        // dst(V16) <- substr(view a, imm0 = 1-based start character, imm1 = character count or -1): UTF-8 aware
+  OP_TS_PART,       // dst(kind: I32, or I64 for TS_SECOND) <- part(aux: TsPart) of timestamp a(I64); imm0 = units per second,
+                    //   imm1 = zone offset from UTC in units
+  OP_TS_TRUNC,      // dst(I64) <- timestamp a(I64) truncated to part (aux) in the zone; imm0 / imm1 as OP_TS_PART
   OP_COUNT_
 };
+// OP_TS_PART / OP_TS_TRUNC parts.  TS_SECOND: the part is the microsecond within the minute, the truncation the whole second;
+// TS_DAYS (part only): local days since the epoch, the cast to Date32.
+enum TsPart : uint16_t { TS_YEAR = 0, TS_QUARTER, TS_MONTH, TS_WEEK, TS_DAY, TS_HOUR, TS_MINUTE, TS_SECOND, TS_DAYS };
 enum : uint16_t { F_IMM_A = 1, F_IMM_B = 2 };
 // OP_CVT source formats (aux)
 enum CvtSrc : uint16_t { SRC_I8 = 0, SRC_I16, SRC_U8, SRC_U16, SRC_U32, SRC_F32, SRC_I32, SRC_I64, SRC_F64, SRC_I128, SRC_B };

@@ -4,10 +4,10 @@
 //! the top of include/sailgpu.h.  Anything that has no spec returns `None`: the node stays a DataFusion node.
 use std::sync::Arc;
 
-use datafusion::arrow::datatypes::DataType;
+use datafusion::arrow::datatypes::{DataType, TimeUnit};
 use datafusion::logical_expr::Operator;
 use datafusion::physical_expr::expressions::{BinaryExpr, CaseExpr, CastExpr, Column, InListExpr, IsNotNullExpr, IsNullExpr, LikeExpr, Literal, NegativeExpr, NotExpr};
-use datafusion::physical_expr::PhysicalExpr;
+use datafusion::physical_expr::{PhysicalExpr, ScalarFunctionExpr};
 use datafusion::physical_plan::aggregates::{AggregateExec, AggregateMode};
 use datafusion::physical_plan::filter::FilterExec;
 use datafusion::physical_plan::joins::{HashJoinExec, NestedLoopJoinExec, PartitionMode};
@@ -28,6 +28,10 @@ pub fn type_name(t: &DataType) -> Option<String> {
         DataType::Date32 => "Date32".into(),
         DataType::Decimal128(p, s) => format!("Decimal128({p},{s})"),
         DataType::Utf8 => "Utf8".into(), DataType::Utf8View => "Utf8View".into(),
+        DataType::Timestamp(u, tz) => {
+            let unit = match u { TimeUnit::Second => "s", TimeUnit::Millisecond => "ms", TimeUnit::Microsecond => "us", TimeUnit::Nanosecond => "ns" };
+            match tz { Some(z) => format!("Timestamp({unit}, {z})"), None => format!("Timestamp({unit})") }
+        }
         _ => return None,
     })
 }
@@ -43,6 +47,8 @@ fn literal(v: &ScalarValue) -> Option<Value> {
         ScalarValue::UInt32(Some(x)) => json!({"lit": x, "type": t}), ScalarValue::UInt64(Some(x)) => json!({"lit": x, "type": t}),
         ScalarValue::Float64(Some(x)) => json!({"lit": x, "type": t}),
         ScalarValue::Date32(Some(x)) => json!({"lit": x, "type": t}),
+        ScalarValue::TimestampSecond(Some(x), _) | ScalarValue::TimestampMillisecond(Some(x), _)
+        | ScalarValue::TimestampMicrosecond(Some(x), _) | ScalarValue::TimestampNanosecond(Some(x), _) => json!({"lit": x, "type": t}),
         ScalarValue::Decimal128(Some(x), _, _) => json!({"lit": x.to_string(), "type": t}), // unscaled integer as text (exact)
         ScalarValue::Utf8(Some(s)) | ScalarValue::Utf8View(Some(s)) => json!({"lit": s, "type": t}),
         _ => return None,
@@ -85,7 +91,19 @@ pub fn expr(e: &Arc<dyn PhysicalExpr>) -> Option<Value> {
         let set: Option<Vec<Value>> = i.list().iter().map(|x| literal(x.as_any().downcast_ref::<Literal>()?.value())).collect();
         return Some(json!({"in": expr(i.expr())?, "set": set?, "negated": i.negated()}));
     }
-    None // ScalarFunctionExpr (date_part, substr): matched by name in `scalar_fn` below
+    if let Some(f) = any.downcast_ref::<ScalarFunctionExpr>() {
+        // date_part / date_trunc with a literal part: DataFusion's simplifier has already folded Sail's part conversion
+        // (`CASE WHEN 'minute' ILIKE ..`) to a literal, as the Partial aggregate's group keys in the ClickBench snapshot show
+        let name = f.name().to_lowercase();
+        if name != "date_part" && name != "date_trunc" { return None; }
+        let [part, arg] = f.args() else { return None };
+        let part = match part.as_any().downcast_ref::<Literal>()?.value() {
+            ScalarValue::Utf8(Some(s)) | ScalarValue::Utf8View(Some(s)) => s.to_lowercase(),
+            _ => return None,
+        };
+        return Some(json!({"fn": name, "part": part, "args": [expr(arg)?]}));
+    }
+    None // other scalar functions (substr, ..) stay DataFusion nodes
 }
 
 pub fn filter(f: &FilterExec) -> Option<Value> {
