@@ -143,3 +143,16 @@ def stored(table: pa.Table) -> pa.Table:
             c = c.cast(pa.int32()).cast(pa.uint16())
         arrays.append(c)
     return pa.table(arrays, names=table.schema.names)
+
+
+def delta_encoding(schema: pa.Schema) -> dict:
+    """pyarrow `column_encoding` for a stored hits table written without dictionaries: integer and timestamp columns as
+    DELTA_BINARY_PACKED, strings as DELTA_BYTE_ARRAY -- the encodings a Parquet V2 writer falls back to when a column outgrows
+    its dictionary.  Write it with `use_dictionary=False, data_page_version="2.0"`."""
+    enc = {}
+    for f in schema:
+        if pa.types.is_integer(f.type) or pa.types.is_timestamp(f.type):
+            enc[f.name] = "DELTA_BINARY_PACKED"
+        elif pa.types.is_binary(f.type) or pa.types.is_string(f.type):
+            enc[f.name] = "DELTA_BYTE_ARRAY"
+    return enc

@@ -205,7 +205,10 @@ SAILGPU_API int32_t sailgpu_spec_validate(const char* spec_json, size_t spec_len
  * annotations): the value stored is the low bytes of the INT32, the truncation parquet-cpp and arrow-rs apply.  The library never
  * sees a BYTE_ARRAY column's annotation, so which Arrow type it decodes to is the caller's choice: a UTF8-annotated column and a
  * plain binary one both decode to Utf8View, bytes passed through unchanged and not validated as UTF-8.  A shim applying
- * `binary_as_string` asks for Utf8View for the binary columns.  Covered: data pages V1/V2, PLAIN and dictionary encodings, flat optional columns,
+ * `binary_as_string` asks for Utf8View for the binary columns.  Covered: data pages V1/V2, PLAIN and dictionary encodings,
+ * DELTA_BINARY_PACKED (INT32 / INT64), DELTA_LENGTH_BYTE_ARRAY (BYTE_ARRAY), DELTA_BYTE_ARRAY (BYTE_ARRAY / FIXED_LEN_BYTE_ARRAY)
+ * and BYTE_STREAM_SPLIT (DOUBLE / INT32 / INT64 / FIXED_LEN_BYTE_ARRAY), mixed freely within a chunk; a corrupt DELTA stream returns
+ * SAILGPU_ERR_INVALID, naming the column (and the page, where the host walk finds it); flat optional columns,
  * uncompressed and ZSTD-compressed pages (codec 0 or 6; columns of both kinds may be mixed in one call); anything else, and
  * ZSTD frames that need a dictionary, returns SAILGPU_ERR_UNSUPPORTED and the caller keeps its CPU reader for that file.
  * ZSTD pages are decompressed on the device by one launch per call, covering every column; the decompressed chunk is read
@@ -223,7 +226,8 @@ typedef struct sailgpu_parquet_column {
 SAILGPU_API int32_t sailgpu_parquet_decode(sailgpu_ctx* ctx, const struct ArrowSchema* schema, const sailgpu_parquet_column* cols,
                                            int32_t n_cols, int64_t n_rows, struct ArrowDeviceArray* out);
 /* Plan-time / diagnostic companion: walks the pages and run headers of column `column` on the host only and reports what it
- * found as JSON ({"pages":..,"dense":non-null values,"dict_count":..,...,"body_bytes":..,"body_fnv1a":..}); fails exactly where
+ * found as JSON ({"pages":..,"dense":non-null values,"dict_count":..,...,"body_bytes":..,"body_fnv1a":..,"delta_pages":..,
+ * "delta_values":..,"bss_pages":..,"bss_values":..}: data pages in a DELTA_* / BYTE_STREAM_SPLIT encoding and their non-null values); fails exactly where
  * sailgpu_parquet_decode would.  body_bytes / body_fnv1a: length and FNV-1a 64 hash of the page bodies walked, in page order,
  * after decompression (a ZSTD chunk is decompressed on the host by the decoder the device runs). */
 SAILGPU_API int32_t sailgpu_parquet_inspect(const struct ArrowSchema* schema, const sailgpu_parquet_column* cols, int32_t n_cols,

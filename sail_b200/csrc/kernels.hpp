@@ -56,6 +56,7 @@ cudaError_t launch_unpack_bits(const uint8_t* bits, uint8_t* bytes, int64_t n, i
 cudaError_t launch_resolve_views(void* views, int64_t n, const uint64_t* bases, cudaStream_t s);
 cudaError_t launch_utf8_to_views(const int32_t* offsets, const uint8_t* bytes, void* views, int64_t n, cudaStream_t s);
 cudaError_t launch_exclusive_scan_u32(const uint32_t* in, int64_t n, uint64_t* out, uint64_t* block_scratch, cudaStream_t s);
+cudaError_t launch_exclusive_scan_u64(const uint64_t* in, int64_t n, uint64_t* out, uint64_t* block_scratch, cudaStream_t s);
 cudaError_t launch_view_lengths(const void* views, int64_t n, uint32_t* lens, int all, cudaStream_t s);
 cudaError_t launch_views_to_arrow(void* views, int64_t n, const uint64_t* offs, uint8_t* heap, cudaStream_t s);
 cudaError_t launch_views_to_utf8(const void* views, int64_t n, const uint64_t* offs, int32_t* out_offsets, uint8_t* heap, cudaStream_t s);

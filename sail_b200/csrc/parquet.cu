@@ -7,10 +7,13 @@
 // decoded on the device.  The host only walks what is inherently sequential and tiny: Thrift page headers and the run
 // headers of the RLE / bit-packed hybrid streams (a few bytes per run); every value is produced by a GPU thread.
 //
-// Covered: data pages V1 / V2, dictionary pages, PLAIN and RLE_DICTIONARY / PLAIN_DICTIONARY values, RLE definition
-// levels of flat optional columns (max level 1), physical types INT32 / INT64 / DOUBLE / FIXED_LEN_BYTE_ARRAY / BYTE_ARRAY,
-// uncompressed and ZSTD-compressed pages.  BOOLEAN, FLOAT and INT96 columns, other codecs, nested columns and the DELTA_*
-// encodings are refused (SAILGPU_ERR_UNSUPPORTED): the caller keeps the CPU reader for those files.
+// Covered: data pages V1 / V2, dictionary pages, PLAIN and RLE_DICTIONARY / PLAIN_DICTIONARY values, DELTA_BINARY_PACKED
+// (INT32 / INT64), DELTA_LENGTH_BYTE_ARRAY (BYTE_ARRAY), DELTA_BYTE_ARRAY (BYTE_ARRAY / FIXED_LEN_BYTE_ARRAY) and
+// BYTE_STREAM_SPLIT (DOUBLE / INT32 / INT64 / FIXED_LEN_BYTE_ARRAY) values, any mix of them in one chunk, RLE definition levels of
+// flat optional columns (max level 1), physical types INT32 / INT64 / DOUBLE / FIXED_LEN_BYTE_ARRAY / BYTE_ARRAY, uncompressed
+// and ZSTD-compressed pages.  BOOLEAN, FLOAT and INT96 columns, other codecs and nested columns are refused
+// (SAILGPU_ERR_UNSUPPORTED): the caller keeps the CPU reader for those files.  Of the DELTA streams the host walks only the
+// block headers (one descriptor per block); one thread per value unpacks its delta and a wrapping 64-bit scan adds them up.
 //
 // INT32 decodes to Int32 / Date32, to Decimal128, and to the narrow integers Int8 / Int16 / UInt8 / UInt16 (how Parquet stores
 // the INT(8|16, signed|unsigned) logical types, e.g. ClickBench's Int16 columns and its UInt16 EventDate): the value kept is the
@@ -92,7 +95,7 @@ struct PageHeader {
   int num_nulls = -1, def_bytes = 0, rep_bytes = 0; bool v2_compressed = true;
 };
 enum { PAGE_DATA = 0, PAGE_DICT = 2, PAGE_DATA_V2 = 3 };
-enum { ENC_PLAIN = 0, ENC_PLAIN_DICT = 2, ENC_RLE = 3, ENC_RLE_DICT = 8 };
+enum { ENC_PLAIN = 0, ENC_PLAIN_DICT = 2, ENC_RLE = 3, ENC_DBP = 5, ENC_DLBA = 6, ENC_DBA = 7, ENC_RLE_DICT = 8, ENC_BSS = 9 };
 enum { PT_BOOLEAN = 0, PT_INT32 = 1, PT_INT64 = 2, PT_INT96 = 3, PT_FLOAT = 4, PT_DOUBLE = 5, PT_BYTE_ARRAY = 6, PT_FLBA = 7 };
 
 PageHeader read_page_header(TReader& r) {
@@ -195,22 +198,89 @@ __global__ void expand_runs_kernel(const uint8_t* __restrict__ chunk, const Run*
   }
 }
 
-// ---- values -> Arrow ------------------------------------------------------------------------------------
-struct Segment { int64_t dense_start; int64_t byte_off; int64_t is_dict; };   // one data page: dense index of its first value, where PLAIN values start, or dictionary-encoded
-struct DecodeParams {
-  const uint8_t* chunk;
-  const uint32_t* valid;            // per row (1 = value present) or null
-  const uint64_t* vpos;             // per row: dense value index (exclusive scan of valid) or null (= row)
-  const uint32_t* dict_idx;         // per dense value: dictionary index, or null (PLAIN)
-  const uint8_t* dict_vals;         // dictionary in Arrow layout (out_width bytes per entry)
-  const Segment* segs; int n_segs;  // PLAIN pages
-  const uint64_t* str_off;          // PLAIN BYTE_ARRAY: byte offset of every dense value's length prefix inside the chunk
-  int64_t n_rows;
-  int physical, type_length, out_width;   // out_width: 1 / 2 (narrow integers from INT32), 4, 8, 16 (Decimal128) or 16 with is_view
-  int is_view;
-  uint32_t dict_size;
+// ---- DELTA_* and BYTE_STREAM_SPLIT pages -> PLAIN layout in a per-column buffer ------------------------------------------
+// Values of these pages are numbered in the column's "decoded" space: the non-null values of its DELTA / BYTE_STREAM_SPLIT
+// pages, in page order.  They are decoded into one buffer, in PLAIN layout (4 / 8 / type_length bytes, or ready 16-byte
+// views for strings), which decode_values_kernel then reads like a PLAIN page.
+constexpr uint32_t ERR_CORRUPT_STREAM = 1u << 8;     // error flag: a DELTA stream the host could not check is corrupt
+
+// One block of a DELTA_BINARY_PACKED stream, walked on the host.  The thread of decoded value i unpacks the delta that leads
+// to the stream's next value, so the stream's values are first_value + an exclusive scan of the deltas.
+struct DeltaBlock {
+  int64_t start;                  // decoded index whose thread unpacks the block's first delta
+  int64_t first, last;            // decoded indices of the stream's first and last value
+  uint64_t first_value, min_delta;
+  uint64_t widths_off, mb_off;    // chunk offsets of the block's miniblock bit widths and of its first miniblock
+  uint64_t per_mb;                // values per miniblock
+};
+// one DELTA / BYTE_STREAM_SPLIT data page in decoded space; data_off / data_len: the BYTE_STREAM_SPLIT values, or the bytes
+// after the length streams of a DELTA_LENGTH_BYTE_ARRAY / DELTA_BYTE_ARRAY page
+struct DecPage { int64_t first, count; uint64_t data_off, data_len; int64_t encoding; };
+
+template <typename T, int64_t T::*Start>
+__device__ __forceinline__ int last_at_or_before(const T* v, int n, int64_t i) {   // last entry that starts at or before i (or 0)
+  int lo = 0, hi = n - 1;
+  while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (v[mid].*Start <= i) lo = mid; else hi = mid - 1; }
+  return lo;
+}
+
+__global__ void delta_unpack_kernel(const uint8_t* __restrict__ chunk, const DeltaBlock* __restrict__ blocks, int n_blocks, int64_t n, uint64_t* __restrict__ deltas) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const DeltaBlock& B = blocks[last_at_or_before<DeltaBlock, &DeltaBlock::start>(blocks, n_blocks, i)];
+    uint64_t d = 0;                                // the stream's last value, and values of no stream, add nothing
+    if (i >= B.start && i < B.last) {
+      const int64_t j = i - B.start;
+      const int64_t m = j / (int64_t)B.per_mb;
+      const uint8_t* w = chunk + B.widths_off;
+      uint64_t bit = 0;
+      for (int64_t k = 0; k < m; ++k) bit += (uint64_t)w[k] * B.per_mb;
+      const uint32_t bw = w[m];
+      bit += (uint64_t)(j - m * (int64_t)B.per_mb) * bw;
+      const uint8_t* p = chunk + B.mb_off + (bit >> 3);
+      uint64_t lo = 0;
+#pragma unroll
+      for (int b = 0; b < 8; ++b) lo |= (uint64_t)p[b] << (8 * b);
+      const int sh = (int)(bit & 7);
+      uint64_t v = lo >> sh;
+      if (sh && bw + sh > 64) v |= (uint64_t)p[8] << (64 - sh);        // 64 value bits + 7 bits of offset: a 9-byte window (buffers are padded)
+      if (bw < 64) v &= (1ull << bw) - 1;
+      d = B.min_delta + v;                         // wrapping: the result is the same whether the writer's deltas were 32- or 64-bit
+    }
+    deltas[i] = d;
+  }
+}
+// value = the stream's first value + the deltas since; stored as its low `width` (4 or 8) bytes.  Values of no stream are left alone.
+__global__ void delta_values_kernel(const DeltaBlock* __restrict__ blocks, int n_blocks, const uint64_t* __restrict__ sums, int64_t n, int width, uint8_t* __restrict__ out) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const DeltaBlock& B = blocks[last_at_or_before<DeltaBlock, &DeltaBlock::start>(blocks, n_blocks, i)];
+    if (i < B.first || i > B.last) continue;
+    const uint64_t v = B.first_value + (sums[i] - sums[B.first]);
+    if (width == 8) reinterpret_cast<uint64_t*>(out)[i] = v;
+    else reinterpret_cast<uint32_t*>(out)[i] = (uint32_t)v;
+  }
+}
+// BYTE_STREAM_SPLIT: byte b of the page's value k sits at b * count + k
+__global__ void byte_stream_split_kernel(const uint8_t* __restrict__ chunk, const DecPage* __restrict__ pages, int n_pages, int64_t n, int width, uint8_t* __restrict__ out) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const DecPage& P = pages[last_at_or_before<DecPage, &DecPage::first>(pages, n_pages, i)];
+    if (P.encoding != ENC_BSS) continue;
+    const uint8_t* src = chunk + P.data_off + (i - P.first);
+    for (int b = 0; b < width; ++b) out[i * width + b] = src[(int64_t)b * P.count];
+  }
+}
+
+struct StringParams {
+  const uint8_t* chunk; const DecPage* pages; int n_pages; int64_t n;
+  const uint32_t* sfx_len; const uint32_t* pfx_len;   // per decoded value: suffix (or whole-value) length, prefix length (0 but in DELTA_BYTE_ARRAY pages)
+  const uint64_t* sfx_pos;                            // exclusive scan of sfx_len
+  const uint64_t* pfx_pos;                            // exclusive scan of pfx_len; null for FIXED_LEN_BYTE_ARRAY
+  uint8_t* heap;                                      // DELTA_BYTE_ARRAY values: at pfx_pos + sfx_pos, or i * type_length
+  ulonglong2* views;                                  // Utf8View output; null for FIXED_LEN_BYTE_ARRAY
+  int type_length;                                    // 0 for BYTE_ARRAY
   uint32_t* error;
 };
+__device__ __forceinline__ uint64_t heap_pos(const StringParams& S, int64_t i) { return S.pfx_pos ? S.pfx_pos[i] + S.sfx_pos[i] : (uint64_t)i * S.type_length; }
+
 __device__ __forceinline__ ulonglong2 make_view(const uint8_t* s, uint32_t len) {
   ulonglong2 v; v.x = len; v.y = 0;
   if (len <= 12) {
@@ -221,6 +291,68 @@ __device__ __forceinline__ ulonglong2 make_view(const uint8_t* s, uint32_t len) 
   }
   return v;
 }
+// every value's suffix, checked against its page: DELTA_LENGTH_BYTE_ARRAY values become views into the chunk, DELTA_BYTE_ARRAY
+// suffixes are copied to the value's place in the heap (its prefix follows in delta_prefix_kernel)
+__global__ void delta_suffix_kernel(StringParams S) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < S.n; i += (int64_t)gridDim.x * blockDim.x) {
+    const DecPage& P = S.pages[last_at_or_before<DecPage, &DecPage::first>(S.pages, S.n_pages, i)];
+    if (P.encoding != ENC_DLBA && P.encoding != ENC_DBA) continue;
+    const uint64_t s = S.sfx_len[i], p = S.pfx_len[i], pos = S.sfx_pos[i] - S.sfx_pos[P.first];
+    const bool last = i == P.first + P.count - 1;
+    if (s > INT32_MAX || p > INT32_MAX || pos + s > P.data_len || (last && pos + s != P.data_len) || (S.type_length && p + s != (uint64_t)S.type_length)) {
+      atomicOr(S.error, ERR_CORRUPT_STREAM);
+      continue;
+    }
+    const uint8_t* src = S.chunk + P.data_off + pos;
+    if (P.encoding == ENC_DLBA) { S.views[i] = make_view(src, (uint32_t)s); continue; }
+    uint8_t* dst = S.heap + heap_pos(S, i) + p;
+    for (uint64_t k = 0; k < s; ++k) dst[k] = src[k];
+  }
+}
+// DELTA_BYTE_ARRAY prefixes, one warp per page (each page starts from an empty previous value): value k's prefix is copied from
+// value k-1's bytes once they are complete, then the page's views are built
+__global__ void delta_prefix_kernel(StringParams S) {
+  const int lane = threadIdx.x & 31;
+  const int64_t gw = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5, nw = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  for (int64_t pg = gw; pg < S.n_pages; pg += nw) {
+    const DecPage P = S.pages[pg];
+    if (P.encoding != ENC_DBA) continue;
+    bool ok = true;
+    for (int64_t i = P.first; i < P.first + P.count; ++i) {
+      const uint64_t p = S.pfx_len[i];
+      const uint64_t prev = i > P.first ? (uint64_t)S.pfx_len[i - 1] + S.sfx_len[i - 1] : 0;
+      if (p > prev || (S.type_length && p + S.sfx_len[i] != (uint64_t)S.type_length)) { ok = false; break; }     // checked before anything is read
+      const uint8_t* src = S.heap + (p ? heap_pos(S, i - 1) : 0);
+      uint8_t* dst = S.heap + heap_pos(S, i);
+      for (uint64_t b = lane; b < p; b += 32) dst[b] = src[b];
+      __syncwarp();
+    }
+    if (!ok) { if (lane == 0) atomicOr(S.error, ERR_CORRUPT_STREAM); continue; }
+    if (S.views)
+      for (int64_t i = P.first + lane; i < P.first + P.count; i += 32) S.views[i] = make_view(S.heap + heap_pos(S, i), S.pfx_len[i] + S.sfx_len[i]);
+  }
+}
+
+// ---- values -> Arrow ------------------------------------------------------------------------------------
+enum { SEG_PLAIN = 0, SEG_DICT = 1, SEG_DECODED = 2 };
+// one data page: dense index of its first value, where its values come from (the chunk, the dictionary or the decoded buffer)
+// and where they start (byte offset inside the chunk, or inside the decoded buffer)
+struct Segment { int64_t dense_start; int64_t byte_off; int64_t kind; };
+struct DecodeParams {
+  const uint8_t* chunk;
+  const uint8_t* decoded;           // values of DELTA / BYTE_STREAM_SPLIT pages in PLAIN layout (views for strings), or null
+  const uint32_t* valid;            // per row (1 = value present) or null
+  const uint64_t* vpos;             // per row: dense value index (exclusive scan of valid) or null (= row)
+  const uint32_t* dict_idx;         // per dense value: dictionary index, or null (PLAIN)
+  const uint8_t* dict_vals;         // dictionary in Arrow layout (out_width bytes per entry)
+  const Segment* segs; int n_segs;  // data pages
+  const uint64_t* str_off;          // PLAIN BYTE_ARRAY: byte offset of every dense value's length prefix inside the chunk
+  int64_t n_rows;
+  int physical, type_length, out_width;   // out_width: 1 / 2 (narrow integers from INT32), 4, 8, 16 (Decimal128) or 16 with is_view
+  int is_view;
+  uint32_t dict_size;
+  uint32_t* error;
+};
 __device__ __forceinline__ void store_plain(const DecodeParams& D, const uint8_t* src, uint8_t* dst) {
   if (D.is_view) {
     uint32_t len; memcpy(&len, src, 4);
@@ -258,7 +390,12 @@ __global__ void decode_values_kernel(DecodeParams D, uint8_t* __restrict__ out) 
     const int64_t v = D.vpos ? (int64_t)D.vpos[i] : i;
     int lo = 0, hi = D.n_segs - 1;               // the page this value came from
     while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (D.segs[mid].dense_start <= v) lo = mid; else hi = mid - 1; }
-    if (D.segs[lo].is_dict) {
+    const Segment& S = D.segs[lo];
+    if (S.kind == SEG_DECODED) {                 // PLAIN layout in the decoded buffer; strings are views already
+      const uint8_t* src = D.decoded + S.byte_off + (v - S.dense_start) * (D.is_view ? 16 : vw);
+      if (D.is_view) *reinterpret_cast<ulonglong2*>(dst) = *reinterpret_cast<const ulonglong2*>(src);
+      else store_plain(D, src, dst);
+    } else if (S.kind == SEG_DICT) {
       const uint32_t k = D.dict_idx[v];
       if (k >= D.dict_size) { atomicOr(D.error, ERR_UNSUPPORTED); continue; }
       const uint8_t* s = D.dict_vals + (size_t)k * D.out_width;       // entries were decoded at the output width
@@ -270,7 +407,7 @@ __global__ void decode_values_kernel(DecodeParams D, uint8_t* __restrict__ out) 
     } else if (D.is_view) {
       store_plain(D, D.chunk + D.str_off[v], dst);
     } else {
-      store_plain(D, D.chunk + D.segs[lo].byte_off + (v - D.segs[lo].dense_start) * vw, dst);
+      store_plain(D, D.chunk + S.byte_off + (v - S.dense_start) * vw, dst);
     }
   }
 }
@@ -331,7 +468,57 @@ struct ColumnPlan {
   const uint8_t* dict_bytes = nullptr;
   bool any_dict_page = false, any_plain_page = false, is_str = false;
   int out_width = 0;
+  // DELTA / BYTE_STREAM_SPLIT pages, in decoded space (see DeltaBlock)
+  std::vector<DecPage> dec_pages;
+  std::vector<DeltaBlock> value_blocks;    // DELTA_BINARY_PACKED values, or the value / suffix lengths of the string encodings
+  std::vector<DeltaBlock> prefix_blocks;   // DELTA_BYTE_ARRAY prefix lengths
+  int64_t decoded = 0, delta_pages = 0, bss_pages = 0, delta_values = 0, bss_values = 0, dba_pages = 0, dlba_pages = 0;
 };
+
+// Walks the DELTA_BINARY_PACKED stream of `count` values at [p, end) of data page `page` into `blocks` (decoded indices from
+// `first`); returns where the stream ends.  The header holds the block size, miniblocks per block, the total count and the
+// first value; every block holds its min delta, one bit width per miniblock and the miniblocks.  No per-value state is kept.
+const uint8_t* walk_delta_stream(const Field& f, int64_t page, const uint8_t* base, const uint8_t* p, const uint8_t* end, int64_t count, int64_t first,
+                                 std::vector<DeltaBlock>* blocks) {
+  const std::string where = "parquet: DELTA_BINARY_PACKED stream of data page " + std::to_string(page) + " of column '" + f.name + "'";
+  auto varint = [&]() -> uint64_t {
+    uint64_t v = 0;
+    for (int sh = 0;; sh += 7) {
+      SG_CHECK(p < end && sh < 64, SAILGPU_ERR_INVALID, where + " overruns its page");
+      const uint8_t b = *p++;
+      v |= (uint64_t)(b & 0x7F) << sh;
+      if (!(b & 0x80)) return v;
+    }
+  };
+  auto zigzag = [&]() -> uint64_t { const uint64_t v = varint(); return (v >> 1) ^ (0 - (v & 1)); };
+  const uint64_t block = varint(), n_mb = varint(), total = varint(), first_value = zigzag();
+  SG_CHECK(block > 0 && block % 128 == 0 && block <= (1u << 30), SAILGPU_ERR_INVALID, where + ": block size " + std::to_string(block) + " is not a multiple of 128");
+  SG_CHECK(n_mb > 0 && block % n_mb == 0 && (block / n_mb) % 32 == 0, SAILGPU_ERR_INVALID,
+           where + ": " + std::to_string(n_mb) + " miniblocks per block of " + std::to_string(block) + " values: values per miniblock must be a multiple of 32");
+  SG_CHECK(total == (uint64_t)count, SAILGPU_ERR_INVALID, where + " holds " + std::to_string(total) + " values, the page " + std::to_string(count));
+  if (count == 0) return p;
+  const uint64_t per_mb = block / n_mb;
+  const int64_t last = first + count - 1;
+  DeltaBlock B{first, first, last, first_value, 0, 0, 0, per_mb};
+  if (count == 1) { blocks->push_back(B); return p; }       // no block follows: the first value is the stream
+  for (int64_t left = count - 1; left > 0; left -= std::min<int64_t>(left, (int64_t)block), B.start += (int64_t)block) {
+    B.min_delta = zigzag();
+    SG_CHECK((uint64_t)(end - p) >= n_mb, SAILGPU_ERR_INVALID, where + " overruns its page");
+    B.widths_off = (uint64_t)(p - base);
+    const uint64_t used = std::min<uint64_t>(n_mb, ((uint64_t)left + per_mb - 1) / per_mb);   // the last block's unused miniblocks have no bodies
+    uint64_t body = 0;
+    for (uint64_t m = 0; m < used; ++m) {
+      SG_CHECK(p[m] <= 64, SAILGPU_ERR_INVALID, where + ": bit width " + std::to_string(p[m]));
+      body += p[m] * per_mb / 8;
+    }
+    p += n_mb;
+    B.mb_off = (uint64_t)(p - base);
+    SG_CHECK((uint64_t)(end - p) >= body, SAILGPU_ERR_INVALID, where + " overruns its page");
+    p += body;
+    blocks->push_back(B);
+  }
+  return p;
+}
 
 void check_parquet_column(const Field& f, const ParquetColumnDesc& c, int64_t n_rows) {
   SG_CHECK(c.codec == CODEC_NONE || c.codec == CODEC_ZSTD, SAILGPU_ERR_UNSUPPORTED,
@@ -455,7 +642,7 @@ ColumnPlan plan_parquet_column(const Field& f, const ParquetColumnDesc& c, int64
     if (h.encoding == ENC_RLE_DICT || h.encoding == ENC_PLAIN_DICT) {
       SG_CHECK(have_dict, SAILGPU_ERR_INVALID, "parquet: dictionary-encoded page without a dictionary page");
       any_dict_page = true;
-      segs.push_back(Segment{dense_done, 0, 1});
+      segs.push_back(Segment{dense_done, 0, SEG_DICT});
       SG_CHECK(vals < body_end || non_null == 0, SAILGPU_ERR_INVALID, "parquet: empty dictionary-index stream");
       if (non_null > 0) {
         const int bw = vals[0];
@@ -465,7 +652,7 @@ ColumnPlan plan_parquet_column(const Field& f, const ParquetColumnDesc& c, int64
       }
     } else if (h.encoding == ENC_PLAIN) {
       any_plain_page = true;
-      segs.push_back(Segment{dense_done, (int64_t)(vals - base), 0});
+      segs.push_back(Segment{dense_done, (int64_t)(vals - base), SEG_PLAIN});
       if (is_str) {
         // offsets are indexed by dense value number: values of earlier DICTIONARY pages get a zero (never read) -- filled
         // only now, so that an all-dictionary chunk keeps no per-value host state at all
@@ -479,6 +666,33 @@ ColumnPlan plan_parquet_column(const Field& f, const ParquetColumnDesc& c, int64
         }
         SG_CHECK(q <= body_end, SAILGPU_ERR_INVALID, "parquet: BYTE_ARRAY value overruns its page");
       }
+    } else if (h.encoding == ENC_DBP || h.encoding == ENC_DLBA || h.encoding == ENC_DBA || h.encoding == ENC_BSS) {
+      const int pt = c.physical_type;
+      const bool ok = h.encoding == ENC_DBP ? (pt == PT_INT32 || pt == PT_INT64)
+                    : h.encoding == ENC_DLBA ? pt == PT_BYTE_ARRAY
+                    : h.encoding == ENC_DBA ? (pt == PT_BYTE_ARRAY || pt == PT_FLBA)
+                    : (pt == PT_INT32 || pt == PT_INT64 || pt == PT_DOUBLE || pt == PT_FLBA);
+      SG_CHECK(ok, SAILGPU_ERR_UNSUPPORTED, "parquet: value encoding " + std::to_string(h.encoding) + " for physical type " + std::to_string(pt) + " (column '" + f.name + "')");
+      const int64_t page = P.n_pages - 1;
+      const std::string where = "parquet: data page " + std::to_string(page) + " of column '" + f.name + "'";
+      const int vw = pt == PT_FLBA ? c.type_length : pt == PT_INT32 ? 4 : 8;
+      segs.push_back(Segment{dense_done, P.decoded * (is_str ? 16 : vw), SEG_DECODED});
+      DecPage dp{P.decoded, non_null, 0, 0, h.encoding};
+      if (h.encoding == ENC_BSS) {
+        SG_CHECK(body_end - vals == non_null * vw, SAILGPU_ERR_INVALID, where + ": BYTE_STREAM_SPLIT values do not fill the page");
+        dp.data_off = (uint64_t)(vals - base); dp.data_len = (uint64_t)(body_end - vals);
+        P.bss_pages++; P.bss_values += non_null;
+      } else {
+        const uint8_t* q = vals;
+        if (h.encoding == ENC_DBA) q = walk_delta_stream(f, page, base, q, body_end, non_null, P.decoded, &P.prefix_blocks);
+        q = walk_delta_stream(f, page, base, q, body_end, non_null, P.decoded, &P.value_blocks);
+        if (h.encoding == ENC_DBP) SG_CHECK(q == body_end, SAILGPU_ERR_INVALID, where + ": the DELTA_BINARY_PACKED stream ends " + std::to_string(body_end - q) + " bytes before the page");
+        dp.data_off = (uint64_t)(q - base); dp.data_len = (uint64_t)(body_end - q);   // the string bytes; the device checks the lengths add up to them
+        P.delta_pages++; P.delta_values += non_null;
+        P.dba_pages += h.encoding == ENC_DBA; P.dlba_pages += h.encoding == ENC_DLBA;
+      }
+      P.dec_pages.push_back(dp);
+      P.decoded += non_null;
     } else fail(SAILGPU_ERR_UNSUPPORTED, "parquet: value encoding " + std::to_string(h.encoding) + " (column '" + f.name + "')");
     rows_done += nv; dense_done += non_null;
   }
@@ -486,6 +700,74 @@ ColumnPlan plan_parquet_column(const Field& f, const ParquetColumnDesc& c, int64
   // (a writer that outgrows its dictionary falls back to PLAIN pages mid-chunk: every page carries its own kind)
 
   return P;
+}
+
+// The values of a column's DELTA / BYTE_STREAM_SPLIT pages, decoded into one buffer in PLAIN layout (16-byte views for strings).
+// A DELTA_BYTE_ARRAY string column also gets a heap holding its rebuilt values, which its views point into.
+BufPtr decode_delta_pages(Ctx* ctx, const ColumnPlan& P, const ParquetColumnDesc& c, const uint8_t* dbase, uint32_t* error, BufPtr* heap) {
+  const int64_t n = P.decoded;
+  const int pt = c.physical_type;
+  const bool lengths = P.is_str || pt == PT_FLBA;     // the DELTA streams hold string lengths, not values
+  const int vw = P.is_str ? 16 : pt == PT_FLBA ? c.type_length : pt == PT_INT32 ? 4 : 8;
+  const int grid = (int)std::min<int64_t>((n + 255) / 256, grid_cap(8));
+  BufPtr out = dev_alloc(ctx, (size_t)n * vw + 64);
+  BufPtr dpages = upload_vec(ctx, P.dec_pages.data(), P.dec_pages.size() * sizeof(DecPage));
+  const DecPage* pages = static_cast<const DecPage*>(dpages->ptr);
+  BufPtr scan_scratch = dev_alloc(ctx, 1026 * 8);
+  // DELTA_BINARY_PACKED: one thread per value unpacks its delta, a wrapping 64-bit scan adds them up
+  auto unpack = [&](const std::vector<DeltaBlock>& blocks, int width, void* dst) {
+    if (blocks.empty()) return;
+    BufPtr dblocks = upload_vec(ctx, blocks.data(), blocks.size() * sizeof(DeltaBlock));
+    BufPtr deltas = dev_alloc(ctx, (size_t)n * 8), sums = dev_alloc(ctx, (size_t)n * 8);
+    const DeltaBlock* b = static_cast<const DeltaBlock*>(dblocks->ptr);
+    delta_unpack_kernel<<<grid, 256, 0, ctx->stream>>>(dbase, b, (int)blocks.size(), n, static_cast<uint64_t*>(deltas->ptr));
+    SG_CUDA(cudaGetLastError());
+    SG_CUDA(launch_exclusive_scan_u64(static_cast<const uint64_t*>(deltas->ptr), n, static_cast<uint64_t*>(sums->ptr), static_cast<uint64_t*>(scan_scratch->ptr), ctx->stream));
+    delta_values_kernel<<<grid, 256, 0, ctx->stream>>>(b, (int)blocks.size(), static_cast<const uint64_t*>(sums->ptr), n, width, static_cast<uint8_t*>(dst));
+    SG_CUDA(cudaGetLastError());
+  };
+  if (P.bss_pages) {
+    byte_stream_split_kernel<<<grid, 256, 0, ctx->stream>>>(dbase, pages, (int)P.dec_pages.size(), n, vw, static_cast<uint8_t*>(out->ptr));
+    SG_CUDA(cudaGetLastError());
+  }
+  if (!lengths) { unpack(P.value_blocks, vw, out->ptr); return out; }
+  if (!P.dba_pages && !P.dlba_pages) return out;
+  // strings: lengths of n values plus a zero, so that the exclusive scans end with their totals
+  BufPtr sfx_len = dev_alloc_zero(ctx, (size_t)(n + 1) * 4), pfx_len = dev_alloc_zero(ctx, (size_t)(n + 1) * 4);
+  BufPtr sfx_pos = dev_alloc(ctx, (size_t)(n + 1) * 8), pfx_pos;
+  unpack(P.value_blocks, 4, sfx_len->ptr);
+  unpack(P.prefix_blocks, 4, pfx_len->ptr);
+  StringParams S; memset(&S, 0, sizeof(S));
+  S.chunk = dbase; S.pages = pages; S.n_pages = (int)P.dec_pages.size(); S.n = n;
+  S.sfx_len = static_cast<const uint32_t*>(sfx_len->ptr); S.pfx_len = static_cast<const uint32_t*>(pfx_len->ptr);
+  S.sfx_pos = static_cast<const uint64_t*>(sfx_pos->ptr); S.error = error;
+  SG_CUDA(launch_exclusive_scan_u32(S.sfx_len, n + 1, static_cast<uint64_t*>(sfx_pos->ptr), static_cast<uint64_t*>(scan_scratch->ptr), ctx->stream));
+  if (P.is_str) {
+    S.views = static_cast<ulonglong2*>(out->ptr);
+    if (P.dba_pages) {                             // the heap: a scan of prefix + suffix lengths, one read-back for its size
+      pfx_pos = dev_alloc(ctx, (size_t)(n + 1) * 8);
+      SG_CUDA(launch_exclusive_scan_u32(S.pfx_len, n + 1, static_cast<uint64_t*>(pfx_pos->ptr), static_cast<uint64_t*>(scan_scratch->ptr), ctx->stream));
+      uint64_t tot[2] = {0, 0};
+      SG_CUDA(cudaMemcpyAsync(&tot[0], static_cast<uint64_t*>(pfx_pos->ptr) + n, 8, cudaMemcpyDeviceToHost, ctx->stream));
+      SG_CUDA(cudaMemcpyAsync(&tot[1], static_cast<uint64_t*>(sfx_pos->ptr) + n, 8, cudaMemcpyDeviceToHost, ctx->stream));
+      stream_sync(ctx);
+      SG_CHECK(tot[0] + tot[1] < (1ull << 40), SAILGPU_ERR_INVALID, "parquet: DELTA_BYTE_ARRAY lengths of a column add up to " + std::to_string(tot[0] + tot[1]) + " bytes");
+      *heap = dev_alloc(ctx, (size_t)(tot[0] + tot[1]) + 64);
+      S.heap = static_cast<uint8_t*>((*heap)->ptr);
+      S.pfx_pos = static_cast<const uint64_t*>(pfx_pos->ptr);
+    }
+  } else {                                         // FIXED_LEN_BYTE_ARRAY: every value is type_length bytes, rebuilt in place
+    S.heap = static_cast<uint8_t*>(out->ptr);
+    S.type_length = c.type_length;
+  }
+  delta_suffix_kernel<<<grid, 256, 0, ctx->stream>>>(S);
+  SG_CUDA(cudaGetLastError());
+  if (P.dba_pages) {
+    const int blocks = (int)std::min<int64_t>(((int64_t)P.dec_pages.size() + 7) / 8, grid_cap(8));
+    delta_prefix_kernel<<<blocks, 256, 0, ctx->stream>>>(S);
+    SG_CUDA(cudaGetLastError());
+  }
+  return out;               // (scratch buffers go back to the stream-ordered pool; the caller syncs before P's host vectors go)
 }
 
 // dimage: for a ZSTD chunk, its image in HBM (c describes the host copy of that image); `image_buf` holds it
@@ -562,6 +844,9 @@ DevColumn decode_parquet_column(Ctx* ctx, const Field& f, const ParquetColumnDes
     didx = expand(index_runs, dense_done);
     D.dict_idx = static_cast<const uint32_t*>(didx->ptr); D.dict_vals = static_cast<const uint8_t*>(ddict->ptr); D.dict_size = (uint32_t)dict_count;
   }
+  BufPtr decoded, heap;
+  if (P.decoded) decoded = decode_delta_pages(ctx, P, c, dbase, D.error, &heap);
+  D.decoded = decoded ? static_cast<const uint8_t*>(decoded->ptr) : nullptr;
   if (is_str && any_plain_page) {
     str_off.resize((size_t)dense_done, 0);
     dstr = upload_vec(ctx, str_off.data(), str_off.size() * 8);
@@ -574,6 +859,7 @@ DevColumn decode_parquet_column(Ctx* ctx, const Field& f, const ParquetColumnDes
   if (n_rows) decode_values_kernel<<<(int)std::min<int64_t>((n_rows + 255) / 256, grid_cap(8)), 256, 0, ctx->stream>>>(D, static_cast<uint8_t*>(col.data->ptr));
   SG_CUDA(cudaGetLastError());
   if (is_str) col.heaps = {dchunk};                 // long views point into the chunk bytes
+  if (is_str && heap) col.heaps.push_back(heap);    // ... or into the values DELTA_BYTE_ARRAY pages rebuilt
   col.null_count = 0;
   if (c.max_def_level > 0 && dense_done < n_rows) {
     // validity bitmap from the expanded levels (u32 0/1 -> bytes -> bits)
@@ -586,6 +872,8 @@ DevColumn decode_parquet_column(Ctx* ctx, const Field& f, const ParquetColumnDes
   uint32_t e = 0;
   SG_CUDA(cudaMemcpyAsync(&e, err->ptr, 4, cudaMemcpyDeviceToHost, ctx->stream));
   stream_sync(ctx);       // host vectors above; error flag
+  SG_CHECK(!(e & ERR_CORRUPT_STREAM), SAILGPU_ERR_INVALID,
+           "parquet: corrupt DELTA_LENGTH_BYTE_ARRAY / DELTA_BYTE_ARRAY values in column '" + f.name + "' (a length overruns its page or differs from the type length, or a prefix is longer than the value before it)");
   SG_CHECK(e == 0, SAILGPU_ERR_INVALID, "parquet: dictionary index out of range in column '" + f.name + "'");
   return col;
 }
@@ -687,9 +975,11 @@ std::string parquet_plan_summary(const Field& f, const ParquetColumnDesc& c, int
   for (auto& s : P.bodies) { body_bytes += s.second; body_hash = fnv1a(body_hash, s.first, s.second); }
   char b[640];
   snprintf(b, sizeof b, "{\"pages\":%lld,\"dense\":%lld,\"dict_count\":%lld,\"level_values\":%lld,\"index_values\":%lld,\"level_runs\":%zu,\"index_runs\":%zu,"
-                        "\"plain_strings\":%zu,\"dict_pages\":%d,\"plain_pages\":%d,\"body_bytes\":%llu,\"body_fnv1a\":%llu}",
+                        "\"plain_strings\":%zu,\"dict_pages\":%d,\"plain_pages\":%d,\"body_bytes\":%llu,\"body_fnv1a\":%llu,"
+                        "\"delta_pages\":%lld,\"delta_values\":%lld,\"bss_pages\":%lld,\"bss_values\":%lld}",      // at most 547 bytes
            (long long)P.n_pages, (long long)P.dense, (long long)P.dict_count, (long long)level_vals, (long long)index_vals, P.level_runs.size(), P.index_runs.size(),
-           P.str_off.size(), P.any_dict_page ? 1 : 0, P.any_plain_page ? 1 : 0, (unsigned long long)body_bytes, (unsigned long long)body_hash);
+           P.str_off.size(), P.any_dict_page ? 1 : 0, P.any_plain_page ? 1 : 0, (unsigned long long)body_bytes, (unsigned long long)body_hash,
+           (long long)P.delta_pages, (long long)P.delta_values, (long long)P.bss_pages, (long long)P.bss_values);
   return b;
 }
 

@@ -2089,9 +2089,10 @@ __global__ void views_to_utf8_kernel(const ulonglong2* __restrict__ views, int64
   }
 }
 
-// exclusive scan of u32 -> u64, single kernel, one CTA walking the array (outputs are small/medium;
+// exclusive scan of u32 or u64 -> u64 (sums wrap modulo 2^64), single kernel, one CTA walking the array (outputs are small/medium;
 // large inputs use chunked partial sums: pass 1 per-block totals, pass 2 applies block offsets)
-__global__ void scan_block_totals_kernel(const uint32_t* __restrict__ in, int64_t n, uint64_t* __restrict__ block_totals, int64_t per_block) {
+template <typename T>
+__global__ void scan_block_totals_kernel(const T* __restrict__ in, int64_t n, uint64_t* __restrict__ block_totals, int64_t per_block) {
   __shared__ unsigned long long ws[32];
   const int64_t b0 = blockIdx.x * per_block, b1 = min(n, b0 + per_block);
   unsigned long long s = 0;
@@ -2101,7 +2102,8 @@ __global__ void scan_block_totals_kernel(const uint32_t* __restrict__ in, int64_
   __syncthreads();
   if (threadIdx.x == 0) { unsigned long long t = 0; for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += ws[w]; block_totals[blockIdx.x] = t; }
 }
-__global__ void scan_apply_kernel(const uint32_t* __restrict__ in, int64_t n, const uint64_t* __restrict__ block_offsets, uint64_t* __restrict__ out, int64_t per_block) {
+template <typename T>
+__global__ void scan_apply_kernel(const T* __restrict__ in, int64_t n, const uint64_t* __restrict__ block_offsets, uint64_t* __restrict__ out, int64_t per_block) {
   // one warp per block-chunk walks sequentially in 32-wide steps (chunks are sized so this is cheap)
   const int64_t b0 = blockIdx.x * per_block, b1 = min(n, b0 + per_block);
   const int lane = threadIdx.x;
@@ -2247,15 +2249,22 @@ __global__ void scan_totals_kernel(uint64_t* t, int64_t nb) {
   }
   if (lane == 0) t[nb] = run;     // grand total after the offsets
 }
-// exclusive scan of u32 lengths into u64 offsets; block_scratch[nblocks] receives the grand total
-cudaError_t launch_exclusive_scan_u32(const uint32_t* in, int64_t n, uint64_t* out, uint64_t* block_scratch /* >= 1025 u64 */, cudaStream_t s) {
+// exclusive scan of u32 lengths (or u64 values, wrapping) into u64 offsets; block_scratch[nblocks] receives the grand total
+template <typename T>
+static cudaError_t launch_exclusive_scan(const T* in, int64_t n, uint64_t* out, uint64_t* block_scratch /* >= 1025 u64 */, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
   const int64_t nblocks = std::min<int64_t>(1024, (n + 4095) / 4096);
   const int64_t per_block = (n + nblocks - 1) / nblocks;
-  scan_block_totals_kernel<<<(int)nblocks, 256, 0, s>>>(in, n, block_scratch, per_block);
+  scan_block_totals_kernel<T><<<(int)nblocks, 256, 0, s>>>(in, n, block_scratch, per_block);
   scan_totals_kernel<<<1, 32, 0, s>>>(block_scratch, nblocks);
-  scan_apply_kernel<<<(int)nblocks, 32, 0, s>>>(in, n, block_scratch, out, per_block);
+  scan_apply_kernel<T><<<(int)nblocks, 32, 0, s>>>(in, n, block_scratch, out, per_block);
   return cudaGetLastError();
+}
+cudaError_t launch_exclusive_scan_u32(const uint32_t* in, int64_t n, uint64_t* out, uint64_t* block_scratch, cudaStream_t s) {
+  return launch_exclusive_scan(in, n, out, block_scratch, s);
+}
+cudaError_t launch_exclusive_scan_u64(const uint64_t* in, int64_t n, uint64_t* out, uint64_t* block_scratch, cudaStream_t s) {
+  return launch_exclusive_scan(in, n, out, block_scratch, s);
 }
 cudaError_t launch_view_lengths(const void* views, int64_t n, uint32_t* lens, int all, cudaStream_t s) {
   if (n == 0) return cudaSuccess;

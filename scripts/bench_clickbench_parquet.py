@@ -10,7 +10,9 @@ Reported: the best of `reps` runs after one warm-up, for the decode (up to resid
 zstd, the decompression launch and the image read-back of that best decode, summed over its row groups (engine.parquet_stats).
 Runs the interpreted pipelines (SAILGPU_JIT=0), as bench.py's ClickBench leg does: the specialised Int16 kernels have not been
 parity-checked on these queries.
-usage: python scripts/bench_clickbench_parquet.py [rows] [reps] [none|zstd]"""
+Layout `plain` (the default) writes what pyarrow writes by default: dictionary pages, falling back to PLAIN.  `delta` writes data
+pages V2 without dictionaries, integer columns as DELTA_BINARY_PACKED and strings as DELTA_BYTE_ARRAY (datagen/hits.py:delta_encoding).
+usage: python scripts/bench_clickbench_parquet.py [rows] [reps] [none|zstd] [plain|delta]"""
 import collections
 import io
 import json
@@ -120,15 +122,22 @@ def main():
     rows = int(sys.argv[1]) if len(sys.argv) > 1 else 10_000_000
     reps = int(sys.argv[2]) if len(sys.argv) > 2 else 5
     codec = sys.argv[3] if len(sys.argv) > 3 else "zstd"
+    layout = sys.argv[4] if len(sys.argv) > 4 else "plain"
     assert codec in ("none", "zstd"), codec
+    assert layout in ("plain", "delta"), layout
     res = {"rows": rows, "codec": codec, "row_group_rows": ROW_GROUP, "card": card()}
+    if layout == "delta":
+        res["layout"] = layout
     print("card", json.dumps(res["card"]), flush=True)
     cols = scanned_columns()
     t0 = time.perf_counter()
     table = gen.hits(rows, seed=11, columns=cols)
     params = sql_params(sql.frame(table.select(["CounterID", "EventDate", "IsRefresh", "TraficSourceID", "DontCountHits", "UserID", "RefererHash", "URLHash"])))
     buf = io.BytesIO()
-    pq.write_table(gen.stored(table), buf, compression=codec, compression_level=3 if codec == "zstd" else None, row_group_size=ROW_GROUP)
+    stored = gen.stored(table)
+    kw = dict(use_dictionary=False, data_page_version="2.0", column_encoding=gen.delta_encoding(stored.schema)) if layout == "delta" else {}
+    pq.write_table(stored, buf, compression=codec, compression_level=3 if codec == "zstd" else None, row_group_size=ROW_GROUP, **kw)
+    del stored
     raw = buf.getvalue()
     del table
     n_groups = pq.ParquetFile(io.BytesIO(raw)).metadata.num_row_groups
