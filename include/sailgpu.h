@@ -151,7 +151,11 @@ enum {
   SAILGPU_ERR_INVALID = 1,      /* bad argument / malformed spec            -> DataFusionError::Plan      */
   SAILGPU_ERR_UNSUPPORTED = 2,  /* type/expression not implemented on GPU   -> DataFusionError::NotImplemented */
   SAILGPU_ERR_CUDA = 3,         /* CUDA / NCCL runtime failure              -> DataFusionError::Execution */
-  SAILGPU_ERR_ARITHMETIC = 4,   /* divide by zero / decimal overflow        -> ArrowError::DivideByZero / ArithmeticOverflow */
+  SAILGPU_ERR_ARITHMETIC = 4,   /* checked arithmetic failed on a row that is evaluated -> ArrowError::DivideByZero / ArithmeticOverflow:
+                                   integer or decimal `/` `%` by zero; integer MIN / -1 and MIN % -1; a decimal `/` `%` whose operand,
+                                   rescaled to the division's scale, leaves i128; avg(Decimal) whose sum * 10^(s_out - s_in) leaves i128.
+                                   `+` `-` `*` and sum() wrap (Int mod 2^64, Decimal128 mod 2^128), as DataFusion's default
+                                   fail_on_overflow = false does, and raise nothing */
   SAILGPU_ERR_NO_DEVICE = 5,    /* no usable CUDA device: there is no CPU fallback */
   SAILGPU_ERR_STATE = 6         /* call sequence violation (push after finish, ...) -> DataFusionError::Internal */
 };

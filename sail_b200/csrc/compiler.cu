@@ -136,8 +136,17 @@ Val PipelineCompiler::compile_bin(const ExprPtr& e) {
       if (op == "/") { const int mp = rt.scale - lt.scale + rt2.scale; lk = mp > 0 ? mp : 0; rk = mp < 0 ? -mp : 0; }
       else { lk = rt.scale - lt.scale; rk = rt.scale - rt2.scale; }
       const int DK = (lt.precision + lk > 18 || rt2.precision + rk > 18 || K == K_I128) ? K_I128 : K_I64;
-      Val a = mul_pow10(convert(l, DK), lk), b = mul_pow10(convert(r, DK), rk);
-      d = emit2(op == "/" ? OP_DIV : OP_REM, DK, DK, a, b, guard_slot(vs));
+      int guard = -2;   // rows evaluated, computed once on first use
+      auto rows_evaluated = [&]() { if (guard == -2) guard = guard_slot(vs); return guard; };
+      auto rescale = [&](const Val& v, int p, int k) {
+        // |v| < 10^p: only where p + k > 38 can the rescale leave i128, and only there is it checked (arrow-rs mul_checked)
+        if (p + k <= 38) return mul_pow10(convert(v, DK), k);
+        Val d = emit2(OP_MUL_POW10_CHK, K_I128, K_I128, ensure_slot(convert(v, K_I128)), imm_pow10(K_I128, k), rows_evaluated());
+        d.vslot = v.vslot;
+        return d;
+      };
+      Val a = rescale(l, lt.precision, lk), b = rescale(r, rt2.precision, rk);
+      d = emit2(op == "/" ? OP_DIV : OP_REM, DK, DK, a, b, rows_evaluated());
       d = convert(d, K);
     }
     d.vslot = vs;
@@ -348,6 +357,9 @@ void PipelineCompiler::finish_aggregate(CompiledPipeline& out, const StageSpec& 
     AccDesc d{}; d.op = (uint8_t)op; d.vkind = (uint8_t)vkind; d.stride = (uint8_t)stride;
     d.value_slot = vslot >= 0 ? (uint32_t)vslot : NO_SLOT; d.valid_slot = valid >= 0 ? (uint32_t)valid : NO_SLOT;
     d.track_seen = (op != ACC_COUNT && (valid >= 0 || A.n_keys == 0)) ? 1 : 0;
+    // a 128-bit min / max is updated by a 16-byte compare-and-swap, which needs a 16-byte aligned address: it starts on an
+    // even word of its entry (and entries are an even number of words long, below)
+    if ((op == ACC_MIN_I128 || op == ACC_MAX_I128) && ((2 + A.key_words + words) & 1)) ++words;
     d.word = (uint16_t)words;
     words += (op == ACC_SUM_I128 || op == ACC_MIN_I128 || op == ACC_MAX_I128) ? 2 : 1;
     A.accs[A.n_accs] = d;
@@ -426,6 +438,9 @@ void PipelineCompiler::finish_aggregate(CompiledPipeline& out, const StageSpec& 
     } else fail(SAILGPU_ERR_UNSUPPORTED, "aggregate function '" + a.fn + "'");
     state_col += at.state.size();
   }
+  bool cas128 = false;
+  for (int j = 0; j < A.n_accs; ++j) cas128 |= A.accs[j].op == ACC_MIN_I128 || A.accs[j].op == ACC_MAX_I128;
+  if (cas128 && ((2 + A.key_words + words) & 1)) ++words;
   A.acc_words = words;
   A.entry_words = (uint32_t)(2 + A.key_words + A.acc_words);
   // thread-private layout: [seen?][one word per accumulator; two for 128-bit min/max]

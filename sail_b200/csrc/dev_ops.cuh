@@ -229,6 +229,22 @@ __device__ __forceinline__ bool fits55(i128 v) {
   return (i128)lo == v && ((uint64_t)(lo + (1ll << 55)) >> 56) == 0;
 }
 
+// checked integer division: MIN / -1 and MIN % -1 have no result in T (arrow-rs div_checked / mod_checked report an
+// overflow for both); a division by zero is reported as such.  Only rows that are evaluated (`live`) raise.
+template <typename T> __device__ __forceinline__ T checked_div(T a, T b, bool rem, bool live, uint32_t* err) {
+  const T min = (T)((u128)1 << (8 * sizeof(T) - 1));
+  if (b == 0) { if (live) atomicOr(err, ERR_DIV_ZERO); return (T)0; }
+  if (b == (T)-1 && a == min) { if (live) atomicOr(err, ERR_OVERFLOW); return (T)0; }
+  return rem ? (T)(a % b) : (T)(a / b);
+}
+
+// a * p for a power of ten p > 1 (decimal rescale up), raising ERR_OVERFLOW for a live row whose product leaves i128.
+// `lim` = I128_MAX / p; p has the factor 5, so it does not divide 2^127 and -lim is the bound below as well.
+__device__ __forceinline__ i128 checked_mul_pow10(i128 a, i128 p, i128 lim, bool live, uint32_t* err) {
+  if ((a > lim || a < -lim) && live) atomicOr(err, ERR_OVERFLOW);
+  return (i128)((u128)a * (u128)p);
+}
+
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 
 __device__ __forceinline__ uint32_t fold32(uint64_t v) { return (uint32_t)v ^ (uint32_t)(v >> 32); }

@@ -642,7 +642,11 @@ struct PipelineOp : Op {
                                 static_cast<unsigned long long*>(nullctr->ptr) + i, ctx->stream));
     }
     SG_CUDA(cudaMemcpyAsync(nulls.data(), nullctr->ptr, (size_t)X.n_cols * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    // the extraction raises an overflow for avg(Decimal) (every such output is nullable, so this read-back covers it)
+    uint32_t err = 0;
+    SG_CUDA(cudaMemcpyAsync(&err, run.scal.error(), 4, cudaMemcpyDeviceToHost, ctx->stream));
     stream_sync(ctx);
+    raise_device_error(ctx, run.scal.error(), err);
     for (int i = 0; i < X.n_cols; ++i) {
       DevColumn& c = out->cols[(size_t)i];
       if (c.validity) { c.null_count = (int64_t)nulls[(size_t)i]; if (c.null_count == 0) c.validity = nullptr; }

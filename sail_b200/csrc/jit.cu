@@ -170,6 +170,14 @@ struct Emitter {
       case OP_MULW: def(I.dst, K_I128, "jit_mulw(" + A(K_I64) + ", " + B(K_I64) + ")"); break;
       case OP_MUL128_64: def(I.dst, K_I128, "jit_mul128_64(" + operand(I.a, K_I128, I.sa) + ", " + B(K_I64) + ")"); break;
       case OP_DIVROUND: def(I.dst, kind, "jit_divround<" + T + ">(" + operand(I.a, kind, I.sa) + ", " + lit(kind, I.imm0, I.imm1) + ")"); break;
+      case OP_MUL_POW10_CHK: {
+        const u128 p = ((u128)I.imm1 << 64) | I.imm0, lim = (~(u128)0 >> 1) / p;
+        std::string live = "inb";
+        if (I.c != NO_SLOT) live += " && " + operand(I.c, K_B, 1);
+        def(I.dst, K_I128, "checked_mul_pow10(" + operand(I.a, K_I128, I.sa) + ", " + lit(K_I128, I.imm0, I.imm1) + ", " +
+                               lit(K_I128, (uint64_t)lim, (uint64_t)(lim >> 64)) + ", " + live + ", K.P[0].error_flag)");
+        break;
+      }
       case OP_EQ: case OP_NE: case OP_LT: case OP_LE: case OP_GT: case OP_GE: {
         if (kind == K_V16) {
           if (base != OP_EQ && base != OP_NE) throw Unsupported{"ordering comparison of strings"};

@@ -69,8 +69,7 @@ template <typename T> __device__ __forceinline__ T jit_divround(T a, T d) {
   return q;
 }
 template <typename T, bool REM> __device__ __forceinline__ T jit_div(T a, T b, bool live, uint32_t* err) {
-  if (b == 0) { if (live) atomicOr(err, ERR_DIV_ZERO); return (T)0; }
-  return REM ? (T)(a % b) : (T)(a / b);
+  return checked_div<T>(a, b, REM, live, err);
 }
 template <typename D, typename S> __device__ __forceinline__ D jit_cvt(S v) {
   // mirrors the interpreter's OP_CVT: integers widen through i128, floats go through int64 towards integers
@@ -517,7 +516,9 @@ __device__ __forceinline__ void jit_agg_reg_tile(const KernelArgs& K, const type
             else {                                               // rare: exact value straight to the table entry
               val[J] = 0;
               uint64_t* e = jit_hot_entry<G>(K, H, gid[k]);
-              if (e) atomic_add_i128(e + 2 + G::KEY_WORDS + G::acc_word(J), a.i);
+              // an Int64 sum has one word and is defined mod 2^64: no carry into the next accumulator
+              if constexpr (G::acc_op(J) == ACC_SUM_I64) { if (e) atomicAdd(reinterpret_cast<unsigned long long*>(e + 2 + G::KEY_WORDS + G::acc_word(J)), (unsigned long long)(int64_t)a.i); }
+              else { if (e) atomic_add_i128(e + 2 + G::KEY_WORDS + G::acc_word(J), a.i); }
             }
           }
         }

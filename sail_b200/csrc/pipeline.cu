@@ -146,13 +146,22 @@ __device__ __noinline__ void vm_div(const VmInst& I, const TileCtx& c, uint32_t*
     T a = (I.flags & F_IMM_A) ? imm : lds<T>(pa + r * I.sa);
     T b = (I.flags & F_IMM_B) ? imm : lds<T>(pb + r * I.sb);
     bool live = r < c.nrows && (pg == nullptr || pg[r]);
-    T q = 0;
-    if (b == 0) {
-      if (live) atomicOr(err, ERR_DIV_ZERO);
-    } else {
-      q = REM ? (T)(a % b) : (T)(a / b);
-    }
-    sts<T>(pd + r * (int)sizeof(T), q);
+    sts<T>(pd + r * (int)sizeof(T), checked_div<T>(a, b, REM, live, err));
+  }
+}
+// decimal rescale up whose product can leave i128 (compiler.cu: checked only where p + k > 38); c = rows evaluated or NO_SLOT
+template <int RPT>
+__device__ __noinline__ void vm_mul_pow10_checked(const VmInst& I, const TileCtx& c, uint32_t* err) {
+  const i128 p = ImmOf<i128>::get(I);
+  const i128 lim = (i128)(~(u128)0 >> 1) / p;
+  const uint8_t* pa = c.arena + eff(c, I.a);
+  const uint8_t* pg = I.c == NO_SLOT ? nullptr : c.arena + eff(c, I.c);
+  uint8_t* pd = c.arena + eff(c, I.dst);
+#pragma unroll
+  for (int k = 0; k < RPT; ++k) {
+    const int r = threadIdx.x + k * NT;
+    const bool live = r < c.nrows && (pg == nullptr || pg[r]);
+    sts<i128>(pd + r * 16, checked_mul_pow10(lds<i128>(pa + r * I.sa), p, lim, live, err));
   }
 }
 template <int RPT>
@@ -603,6 +612,7 @@ __device__ __forceinline__ void vm_exec(const VmInst* prog, int n_inst, const Ti
       case OP_DIVROUND:
         if (kind == K_I64) vm_divround<RPT, int64_t>(I, c); else vm_divround<RPT, i128>(I, c);
         break;
+      case OP_MUL_POW10_CHK: vm_mul_pow10_checked<RPT>(I, c, P.error_flag); break;
       case OP_EQ: if (kind == K_V16) vm_view_eq<RPT>(I, c, false); else vm_cmp_kind<RPT, CmpEq>(I, kind, c); break;
       case OP_NE: if (kind == K_V16) vm_view_eq<RPT>(I, c, true); else vm_cmp_kind<RPT, CmpNe>(I, kind, c); break;
       case OP_LT: vm_cmp_kind<RPT, CmpLt>(I, kind, c); break;
@@ -1295,7 +1305,12 @@ __device__ __forceinline__ void sink_agg_reg(const PipelineParams& P, const AggP
             if (fits55(x)) val[j] = (int64_t)x;
             else {                                            // rare: exact value straight to the table entry
               uint64_t* e = hot_entry(P, A, H, gid[k]);
-              if (e) atomic_add_i128(e + 2 + A.key_words + A.accs[j].word, x);
+              if (e) {
+                uint64_t* dst = e + 2 + A.key_words + A.accs[j].word;
+                // an Int64 sum has one word and is defined mod 2^64: no carry into the next accumulator
+                if (A.accs[j].op == ACC_SUM_I64) atomicAdd(reinterpret_cast<unsigned long long*>(dst), (unsigned long long)(int64_t)x);
+                else atomic_add_i128(dst, x);
+              }
             }
           }
         }
@@ -1987,11 +2002,15 @@ __global__ void agg_extract_kernel(AggParams A, AggExtractParams X, uint64_t n_g
           double sum = __longlong_as_double((long long)aw[ds.word]);
           *reinterpret_cast<double*>(dst) = valid ? sum / (double)cnt : 0.0;
         } else {
-          // DecimalAverager: (sum * 10^(s_out - s_in)) / count, truncating toward zero
+          // DecimalAverager: (sum * 10^(s_out - s_in)) / count, truncating toward zero; a product that leaves i128 is an
+          // overflow error ("Arithmetic Overflow in AvgAccumulator")
           i128 sum = acc_words_of(ds.op) == 2 ? (i128)(((u128)aw[ds.word + 1] << 64) | aw[ds.word]) : (i128)(int64_t)aw[ds.word];
           i128 mul = (i128)(((u128)o.scale_mul_hi << 64) | o.scale_mul_lo);
           i128 q = 0;
-          if (valid) q = (sum * mul) / (i128)cnt;
+          if (valid) {
+            if (mul > 1) { const i128 lim = (i128)(~(u128)0 >> 1) / mul; if (sum > lim || sum < -lim) atomicOr(err, ERR_OVERFLOW); }
+            q = (i128)((u128)sum * (u128)mul) / (i128)cnt;
+          }
           reinterpret_cast<uint64_t*>(dst)[0] = (uint64_t)(u128)q; reinterpret_cast<uint64_t*>(dst)[1] = (uint64_t)((u128)q >> 64);
         }
       }
