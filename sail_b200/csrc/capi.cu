@@ -326,8 +326,15 @@ SAILGPU_API int64_t sailgpu_op_metrics(sailgpu_op* h, char* json_buf, size_t cap
                    (unsigned long long)h->op->pipeline_kernel_ns(), (unsigned long long)h->owner->ctx.exch_sent_bytes.load(),
                    (unsigned long long)h->owner->ctx.exch_recv_bytes.load(), (unsigned long long)h->owner->ctx.exch_ns.load(),
                    (unsigned long long)h->owner->ctx.exch_calls.load(), (unsigned long long)m.host_syncs);
-  if (json_buf && cap) { size_t k = std::min<size_t>((size_t)n, cap - 1); memcpy(json_buf, tmp, k); json_buf[k] = 0; }
-  return n + 1;
+  std::string js(tmp, (size_t)std::max(0, std::min(n, (int)sizeof(tmp) - 1)));
+  if (m.agg_spills) {      // an aggregate that went into partitioned mode
+    js.pop_back();
+    js += ",\"gpu.agg_spills\":" + std::to_string(m.agg_spills) + ",\"gpu.agg_partitions\":" + std::to_string(m.agg_partitions) + ",\"gpu.agg_partition_groups\":[";
+    for (size_t i = 0; i < m.agg_partition_groups.size(); ++i) js += (i ? "," : "") + std::to_string(m.agg_partition_groups[i]);
+    js += "]}";
+  }
+  if (json_buf && cap) { size_t k = std::min<size_t>(js.size(), cap - 1); memcpy(json_buf, js.data(), k); json_buf[k] = 0; }
+  return (int64_t)js.size() + 1;
 }
 
 SAILGPU_API const char* sailgpu_last_error(const sailgpu_op* h) { return h ? h->last_error.c_str() : "null handle"; }

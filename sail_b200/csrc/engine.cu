@@ -180,14 +180,20 @@ struct PipelineOp : Op {
   bool pull(BatchPtr* out) override {
     *out = nullptr;
     if (has_agg) {
-      if (!input_done) return true;
-      if (emitted) return false;
-      const uint64_t t0 = now_ns();
-      *out = extract_agg();
-      m.elapsed_compute_ns += now_ns() - t0;
-      emitted = true;
-      m.output_rows += (uint64_t)(*out)->rows; m.output_batches++;
-      return false;
+      // the aggregate's result once the input ended; before that only what partitioned mode emitted early (partial mode)
+      if (input_done && !emitted) {
+        const uint64_t t0 = now_ns();
+        if (tab.capacity) current_groups();      // resolves the launches in flight first: they may still spill
+        if (spilled.empty()) ready.push_back(extract_agg());
+        else finish_partitioned();
+        m.elapsed_compute_ns += now_ns() - t0;
+        emitted = true;
+      }
+      if (!ready.empty()) {
+        *out = ready.front(); ready.pop_front();
+        m.output_rows += (uint64_t)(*out)->rows; m.output_batches++;
+      }
+      return !(emitted && ready.empty());
     }
     if (!ready.empty()) {
       *out = ready.front(); ready.pop_front();
@@ -271,6 +277,13 @@ struct PipelineOp : Op {
   static constexpr uint64_t MIN_CAPACITY = 1ull << 22, MAX_CAPACITY = 1ull << 28;
   static constexpr uint64_t CARD_MANY_GROUPS = 256, HOT_GROUP_LIMIT = 1 << 16;
   static uint64_t min_capacity() { const char* v = getenv("SAILGPU_AGG_MIN_CAPACITY"); return v && *v ? next_pow2((uint64_t)atoll(v)) : MIN_CAPACITY; }
+  // the most slots one table may have (tests lower it, so that partitioned mode is reached with few groups); the table of a
+  // partition of partitioned mode (below) is sized to stay under MAX_CAPACITY whatever the ceiling was
+  bool partition_of_parent = false;
+  uint64_t max_capacity() const {
+    const char* v = getenv("SAILGPU_AGG_MAX_CAPACITY");
+    return v && *v && !partition_of_parent ? std::min(MAX_CAPACITY, next_pow2((uint64_t)atoll(v))) : MAX_CAPACITY;
+  }
   bool use_cold = false;
   int64_t rows_in_table = 0;
   int64_t known_groups = -1;      // group count read (and error flag checked) once nothing was in flight any more, -1 = stale
@@ -478,7 +491,7 @@ struct PipelineOp : Op {
     const bool grouped = cp->agg.n_keys > 0;
     // first table: 4 M slots for real inputs, but a final aggregate over a few partial rows gets a few KB (a hand-back
     // grows it if later batches are bigger)
-    if (!tab.capacity) alloc_table(cp->agg, grouped ? std::min<uint64_t>(min_capacity(), next_pow2(8 * (uint64_t)b->rows + 2048)) : 1024, 0);
+    if (!tab.capacity) alloc_table(cp->agg, grouped ? std::min<uint64_t>(std::min<uint64_t>(min_capacity(), max_capacity()), next_pow2(8 * (uint64_t)b->rows + 2048)) : 1024, 0);
     const int64_t tile_rows = (int64_t)cp->rpt * NT;
     const int64_t n_tiles = (b->rows + tile_rows - 1) / tile_rows;
     BufPtr deferred = grouped ? dev_alloc(ctx, (size_t)n_tiles * 4) : nullptr;
@@ -536,6 +549,18 @@ struct PipelineOp : Op {
       const bool stuck = prev_def != 0 && n_def_total >= prev_def;
       if (cap <= tab.capacity && stuck) cap = tab.capacity * 2;
       prev_def = n_def_total;
+      // partitioned mode: the table grows to the ceiling and no further.  A full table at the ceiling hands its groups on as
+      // state rows (spill) and starts over empty; the re-launches below then fill it again.
+      const uint64_t ceiling = max_capacity();
+      if (cap > ceiling) {
+        cap = ceiling;
+        if (tab.capacity >= ceiling && groups) {
+          SG_CHECK(!partition_of_parent, SAILGPU_ERR_UNSUPPORTED, "a partition of a partitioned aggregate needs more than 2^28 group slots");
+          spill(groups);
+          rows_in_table = (int64_t)rows_def;
+          prev_def = 0;
+        }
+      }
       if (cap > tab.capacity) alloc_table(inflight.front().cp->agg, cap, groups);
       if (!use_cold && groups > CARD_MANY_GROUPS && getenv("SAILGPU_NO_COLD") == nullptr) {
         auto cold = run.compiled_for(*inflight.front().batch, true);
@@ -583,19 +608,25 @@ struct PipelineOp : Op {
       for (auto& f : run.in_schema) { DevColumn c; c.type = f.type; dummy.cols.push_back(c); }
       cp = run.compiled_for(dummy);
     }
-    const AggParams& A0 = cp->agg;
     run.ensure_scratch();
     const uint64_t groups = tab.capacity ? current_groups() : 0;
+    return extract_rows(*cp, cp->agg_outs, groups);
+  }
+
+  // the table's `groups` groups as the columns `outs` describe (the operator's output, or the state rows of partitioned mode)
+  BatchPtr extract_rows(const CompiledPipeline& cp, const std::vector<AggOutSpec>& outs, uint64_t groups) {
+    const AggParams& A0 = cp.agg;
+    run.ensure_scratch();
     const bool synth = A0.n_keys == 0 && groups == 0;   // global aggregate over zero rows: one row of NULLs / zero counts
     const int64_t rows = synth ? 1 : (int64_t)groups;
     auto out = std::make_shared<DevBatch>();
     out->rows = rows;
     AggExtractParams X;
     memset(&X, 0, sizeof(X));
-    X.n_cols = (int)cp->agg_outs.size();
+    X.n_cols = (int)outs.size();
     std::vector<BufPtr> vbytes((size_t)X.n_cols);
     for (int i = 0; i < X.n_cols; ++i) {
-      const AggOutSpec& s = cp->agg_outs[(size_t)i];
+      const AggOutSpec& s = outs[(size_t)i];
       AggOutCol& o = X.cols[i];
       o.kind = s.kind; o.a = s.a; o.b = s.b; o.nullable = s.nullable ? 1 : 0;
       o.width = s.type.is_string() ? 16 : s.type.arrow_width();
@@ -622,7 +653,7 @@ struct PipelineOp : Op {
     } else if (synth) {
       // counts are 0 (valid); every other aggregate is NULL -> validity bytes stay 0, count columns get no validity
       for (int i = 0; i < X.n_cols; ++i) {
-        const AggOutSpec& s = cp->agg_outs[(size_t)i];
+        const AggOutSpec& s = outs[(size_t)i];
         const bool is_count = s.kind == 1 && (A0.accs[s.a].op == ACC_COUNT || (A0.accs[s.a].op == ACC_SUM_I64 && !A0.accs[s.a].track_seen));
         if (vbytes[(size_t)i] && is_count) SG_CUDA(cudaMemsetAsync(vbytes[(size_t)i]->ptr, 1, 1, ctx->stream));
       }
@@ -652,6 +683,120 @@ struct PipelineOp : Op {
       if (c.validity) { c.null_count = (int64_t)nulls[(size_t)i]; if (c.null_count == 0) c.validity = nullptr; }
     }
     return out;
+  }
+
+  // ---- partitioned mode ------------------------------------------------------------------------
+  // A table at the ceiling (max_capacity) that would have to grow hands its groups on as partial-aggregate state rows and
+  // starts over.  A partial aggregate emits those rows right away (the final aggregate after it merges a group emitted more
+  // than once).  The other modes keep them in HBM; when the input has ended, the rows still in the table join them, they
+  // are hash-partitioned on the group key by RepartitionOp, and one final aggregate per partition merges each partition's
+  // rows in a table of its own.  Aggregates whose table stays under the ceiling never get here.
+  std::vector<BatchPtr> spilled;
+
+  // State rows as a partial aggregate emits them: keys, then each aggregate's state columns.  Every mode's table holds the
+  // accumulators of those states (compiler.cu finish_aggregate: single and partial compile the same accumulators, the final
+  // modes merge state columns into accumulators of the same kinds, avg as a count and a sum, Decimal128 sums in 128 bits);
+  // only the outputs differ, where avg is sum / count.
+  static std::vector<AggOutSpec> state_outs(const CompiledPipeline& cp) {
+    std::vector<AggOutSpec> outs;
+    for (const AggOutSpec& s : cp.agg_outs) {
+      if (s.kind != 2) { outs.push_back(s); continue; }
+      AggOutSpec c = s, v = s;
+      c.kind = 1; c.a = s.b; c.b = 0; c.type = T(TypeId::UInt64); c.nullable = false;
+      v.kind = 1; v.b = 0; v.type = agg_types("avg", s.in_type).state[1]; v.nullable = cp.agg.accs[s.a].track_seen != 0;
+      outs.push_back(c); outs.push_back(v);
+    }
+    return outs;
+  }
+
+  void spill(uint64_t groups) {
+    Trace tr(ctx, "agg.spill");
+    BatchPtr rows = extract_rows(*agg_cp, state_outs(*agg_cp), groups);
+    if (tab.direct) { AggParams A = agg_cp->agg; fill_table(A); SG_CUDA(launch_agg_init_direct(A, ctx->stream)); m.kernel_launches++; }
+    else SG_CUDA(cudaMemsetAsync(tab.state->ptr, 0, (size_t)tab.capacity * 4, ctx->stream));
+    SG_CUDA(cudaMemsetAsync(run.scal.n_groups(), 0, 8, ctx->stream));
+    known_groups = -1;
+    m.agg_spills++;
+    if (run.stages.back().mode == "partial") ready.push_back(rows);
+    else spilled.push_back(rows);
+  }
+
+  static Json jnum(int64_t v) { Json j; j.kind = Json::Num; j.s = std::to_string(v); return j; }
+  static Json jstr(const std::string& v) { Json j; j.kind = Json::Str; j.s = v; return j; }
+  static Json jcol(int64_t i) { Json j; j.kind = Json::Obj; j.o = {{"col", jnum(i)}}; return j; }
+
+  // the end of the input in partitioned mode (single / final / final_partitioned): one output batch per partition
+  void finish_partitioned() {
+    Trace tr(ctx, "agg.partitions");
+    const std::shared_ptr<CompiledPipeline> cp = agg_cp;
+    const uint64_t left = current_groups();
+    if (left) spilled.push_back(extract_rows(*cp, state_outs(*cp), left));
+    const StageSpec& st = run.stages.back();
+    const int n_keys = (int)st.group_exprs.size();
+    Schema states;
+    const std::vector<AggOutSpec> souts = state_outs(*cp);
+    for (size_t i = 0; i < souts.size(); ++i)
+      states.push_back({i < (size_t)n_keys ? out_schema[i].name : "__state" + std::to_string(i), souts[i].type, souts[i].nullable || (i < (size_t)n_keys && out_schema[i].nullable)});
+    uint64_t rows = 0;
+    for (auto& b : spilled) rows += (uint64_t)b->rows;
+    // P: the smallest power of two that leaves at most an eighth of the ceiling's slots in state rows per partition.  A
+    // partition's rows bound its groups, so its table ends at most a quarter full and never reaches the ceiling itself.
+    const uint64_t per_part = std::max<uint64_t>(1, max_capacity() / 8);
+    uint64_t n_parts = 1;
+    while (n_parts * per_part < rows) n_parts *= 2;
+    SG_CHECK(n_parts <= 4096, SAILGPU_ERR_UNSUPPORTED, "aggregate needs more than 4096 key-hash partitions");
+    std::vector<std::vector<BatchPtr>> parts((size_t)n_parts);
+    if (n_parts == 1) parts[0].swap(spilled);
+    else {
+      // the partition of a row is RepartitionOp's hash of the key values (nulls and string contents, not views) modulo P: the
+      // low bits of a hash that the group table's probe (pipeline.cu hash_packed_key: another seed, another mixing chain) does
+      // not share, so every partition's keys still spread over all slots of its table
+      Json keys; keys.kind = Json::Arr;
+      for (int i = 0; i < n_keys; ++i) keys.a.push_back(jcol(i));
+      Json spec; spec.kind = Json::Obj;
+      spec.o = {{"op", jstr("repartition")}, {"scheme", jstr("hash")}, {"exprs", keys}, {"n", jnum((int64_t)n_parts)}};
+      std::unique_ptr<Op> rp = make_op(ctx, spec, {states}, 0);
+      for (auto& b : spilled) rp->push(0, b);
+      spilled.clear();
+      rp->finish(0);
+      for (uint64_t p = 0; p < n_parts; ++p)
+        for (;;) { BatchPtr b; const bool more = rp->pull_partition((int)p, &b); if (b && b->rows) parts[(size_t)p].push_back(b); if (!more) break; }
+      m.kernel_launches += rp->m.kernel_launches;
+    }
+    // one final aggregate per partition over the state rows: [keys | states] -> the operator's output
+    Json gb; gb.kind = Json::Arr;
+    for (int i = 0; i < n_keys; ++i) { Json g; g.kind = Json::Obj; g.o = {{"expr", jcol(i)}, {"name", jstr(st.group_names[(size_t)i])}}; gb.a.push_back(g); }
+    Json aggs; aggs.kind = Json::Arr;
+    for (auto& a : st.aggs) {
+      Json j; j.kind = Json::Obj;
+      j.o = {{"fn", jstr(a.fn)}, {"name", jstr(a.name)}};
+      if (a.input_type.id != TypeId::Null) j.o.push_back({"input_type", jstr(a.input_type.str())});
+      aggs.a.push_back(j);
+    }
+    Json fspec; fspec.kind = Json::Obj;
+    fspec.o = {{"op", jstr("aggregate")}, {"mode", jstr("final")}, {"group_by", gb}, {"aggs", aggs}};
+    m.agg_partition_groups.assign((size_t)n_parts, 0);
+    for (uint64_t p = 0; p < n_parts; ++p) {
+      std::vector<BatchPtr> in;
+      in.swap(parts[(size_t)p]);
+      if (in.empty()) continue;
+      std::unique_ptr<Op> op = make_op(ctx, fspec, {states}, 0);
+      PipelineOp* po = dynamic_cast<PipelineOp*>(op.get());
+      SG_CHECK(po != nullptr, SAILGPU_ERR_STATE, "partitioned aggregate: the per-partition aggregate is not a hash aggregate");
+      po->partition_of_parent = true;
+      for (auto& b : in) op->push(0, b);
+      in.clear();
+      op->finish(0);
+      std::vector<BatchPtr> outs;
+      for (;;) { BatchPtr o; const bool more = op->pull(&o); if (o && o->rows) outs.push_back(o); if (!more) break; }
+      m.kernel_launches += op->m.kernel_launches;
+      if (outs.empty()) continue;
+      BatchPtr o = outs.size() == 1 ? outs[0] : concat_batches(ctx, out_schema, outs);
+      m.agg_partition_groups[(size_t)p] = (uint64_t)o->rows;
+      ready.push_back(o);
+    }
+    m.agg_partitions = n_parts;
+    if (ready.empty()) ready.push_back(empty_batch(ctx, out_schema));
   }
 };
 

@@ -17,6 +17,10 @@ struct Metrics {
   uint64_t build_input_rows = 0, build_input_batches = 0, build_time_ns = 0, join_time_ns = 0;
   uint64_t pipeline_launches = 0, pipeline_kernel_ns = 0, jit_launches = 0;
   uint64_t host_syncs = 0;      // stream drains during calls on this operator's handle (import and export included), capi.cu
+  // partitioned mode of a hash aggregate (engine.cu): times the table was emptied at its ceiling, key-hash partitions, groups
+  // each partition's final aggregate produced
+  uint64_t agg_spills = 0, agg_partitions = 0;
+  std::vector<uint64_t> agg_partition_groups;
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> pending;   // CUDA events bracketing each pipeline-kernel launch
 };
 

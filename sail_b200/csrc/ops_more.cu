@@ -1163,7 +1163,7 @@ struct WideAggOp : Op {
   std::vector<BatchPtr> parts;
   bool input_done = false, emitted = false;
   int n_keys = 0;
-  bool merging = false;
+  bool merging = false, partial = false;
 
   static Json jnum(int64_t v) { Json j; j.kind = Json::Num; j.s = std::to_string(v); return j; }
   static Json jstr(const std::string& v) { Json j; j.kind = Json::Str; j.s = v; return j; }
@@ -1276,7 +1276,8 @@ struct WideAggOp : Op {
     }
     Schema aos;
     BatchPtr agg = through(jobj(so2), ain, agg_in, &aos);
-    SG_CHECK((uint64_t)agg->rows == n_groups, SAILGPU_ERR_STATE, "sort-based grouping: group count mismatch");
+    // a partial aggregate in partitioned mode may emit a group more than once
+    SG_CHECK((uint64_t)agg->rows == n_groups || (partial && (uint64_t)agg->rows > n_groups), SAILGPU_ERR_STATE, "sort-based grouping: group count mismatch");
     // 5. key columns of the result: the representative row of each output group
     JoinOp helper; helper.ctx = ctx;
     DevColumn repc; repc.type = T(TypeId::Int64); repc.length = (int64_t)n_groups; repc.data = rep;
@@ -1300,6 +1301,7 @@ std::unique_ptr<Op> make_wide_agg_op(Ctx* ctx, const Json& spec, const std::vect
   op->n_keys = (int)spec.at("group_by").a.size();
   const std::string mode = spec.at("mode").as_str();
   op->merging = mode == "final" || mode == "final_partitioned";
+  op->partial = mode == "partial";
   SG_CHECK(op->n_keys >= 1 && op->n_keys <= 7, SAILGPU_ERR_UNSUPPORTED, "sort-based grouping takes 1 to 7 group keys");
   for (int i = 0; i < op->n_keys; ++i) {
     const DataType& t = out_schema[(size_t)i].type;

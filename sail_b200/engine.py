@@ -309,7 +309,10 @@ class GpuExec:
 
     def metrics(self) -> dict:
         buf = ctypes.create_string_buffer(2048)
-        lib().sailgpu_op_metrics(self._h, buf, 2048)
+        need = lib().sailgpu_op_metrics(self._h, buf, 2048)
+        if need > 2048:      # a partitioned aggregate lists the groups of every partition
+            buf = ctypes.create_string_buffer(need)
+            lib().sailgpu_op_metrics(self._h, buf, need)
         return json.loads(buf.value.decode())
 
     def collect(self) -> pa.Table:
