@@ -64,6 +64,8 @@
  *                                           Decimal128(8,6), the microsecond within the minute; in the column's zone)
  *   {"fn":"date_trunc","part":"year|quarter|month|week|day|hour|minute|second","args":[E]}   (E Timestamp -> its type)
  *   {"fn":"substr","args":[E],"start":s,"length":n|null}   (1-based, in characters)
+ *   {"fn":"character_length","args":[E]}   (E Utf8 / Utf8View -> Int32: the bytes that are not UTF-8 continuation bytes,
+ *                                           i.e. the characters of valid UTF-8; NULL for NULL)
  * Types T: Boolean Int8..Int64 UInt8..UInt64 Float32 Float64 Date32 Decimal128(p,s) Utf8 Utf8View
  *   Timestamp(s|ms|us|ns[, zone]) (Arrow tss: / tsm: / tsu: / tsn: + zone; stored as Int64).  Any zone passes through the
  *   operators; date_part, date_trunc and the cast to Date32 read wall-clock time and accept no zone, UTC or +HH:MM / -HH:MM

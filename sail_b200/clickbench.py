@@ -12,7 +12,8 @@ nothing falls back):
   18, 42  extract(minute ..) / date_trunc('minute', ..) on a Timestamp: planned in TIMESTAMP_QUERIES (over the Int64 EventTime of
           the view, cast to Timestamp(us, UTC) as the reference's scan projection does)
   21, 22  MIN(URL) / MIN(Title): min/max over strings (planned below as REJECTED, the tests pin the plan-time error)
-  27, 28  length() / regexp_replace(): scalar string functions outside {substr, like}
+  27      length(URL): character_length, planned in LENGTH_QUERIES
+  28      regexp_replace(): a scalar string function outside {substr, like, character_length}
 Strings are Utf8View and EventTime is Int64 seconds (see datagen/hits.py); [23] `SELECT *` selects ten columns, [29] runs as six aggregates.
 """
 from __future__ import annotations
@@ -20,7 +21,7 @@ from __future__ import annotations
 from dataclasses import dataclass
 from typing import Callable
 
-from .plans import Node, aggregate, and_, binop, col, date, filter_, like, lit, project, scan, sort, string, two_phase
+from .plans import Node, aggregate, and_, binop, char_length, col, date, filter_, like, lit, project, scan, sort, string, two_phase
 
 I16, I32, I64 = "Int16", "Int32", "Int64"
 COUNT_STAR = ("count", None, "c", None)
@@ -315,6 +316,14 @@ def c42(skip=1000):
     return sort(a, [("M", True)], fetch=skip + 10)
 
 
+def c27(min_count: int = 100000):
+    """avg(length(URL)) per CounterID: Spark's `length` is DataFusion's `character_length` in both the Partial and the
+    FinalPartitioned aggregate (test_clickbench.plan.yaml [27]); HAVING is a filter on the final count"""
+    f = filter_(hits(["CounterID", "URL"]), ne_empty("URL"))
+    a = two_phase(f, ["CounterID"], [("avg", char_length(col("URL")), "l", I32), COUNT_STAR])
+    return sort(filter_(a, binop(">", col("c"), lit(min_count, I64))), [("l", False)], fetch=25)
+
+
 @dataclass
 class Query:
     plan: Callable[..., Node]
@@ -359,5 +368,7 @@ QUERIES = {
 REJECTED = {"c21": Query(c21, 21, order=("c",)), "c22": Query(c22, 22, order=("c",))}
 # the two queries that need the Timestamp type: planned here, outside QUERIES, so that the split above stays as the tests pin it
 TIMESTAMP_QUERIES = {"c18": Query(c18, 18, order=("count(*)",)), "c42": Query(c42, 42, order=("M",), skip=1000)}
-NOT_PLANNED = {18: "extract(minute FROM Timestamp): TIMESTAMP_QUERIES['c18']", 27: "length(URL)", 28: "regexp_replace(Referer, ..)",
+# [27] needs character_length: planned outside QUERIES as well
+LENGTH_QUERIES = {"c27": Query(c27, 27, order=("l",), floats=(1,), params=("min_count",))}
+NOT_PLANNED = {18: "extract(minute FROM Timestamp): TIMESTAMP_QUERIES['c18']", 27: "length(URL): LENGTH_QUERIES['c27']", 28: "regexp_replace(Referer, ..)",
                42: "date_trunc('minute', Timestamp): TIMESTAMP_QUERIES['c42']"}

@@ -294,6 +294,15 @@ Val PipelineCompiler::compile_uncached(const ExprPtr& e) {
       out.vslot = a.vslot;
       return out;
     }
+    case Expr::CharLength: {
+      Val a = ensure_slot(compile(e->args[0]));
+      Val out = temp(K_I32);
+      VmInst I{}; I.op = (uint16_t)(OP_CHAR_LEN | (K_I32 << 8)); I.dst = (uint32_t)out.slot; I.a = (uint32_t)a.slot; I.b = I.c = NO_SLOT;
+      I.sa = (uint8_t)a.stride;
+      prog_.push_back(I);
+      out.vslot = a.vslot;
+      return out;
+    }
     case Expr::DateTrunc: {
       const DataType& t = e->args[0]->type;
       return ts_op(OP_TS_TRUNC, K_I64, timestamp_part("date_trunc", e->op), compile(e->args[0]), t);

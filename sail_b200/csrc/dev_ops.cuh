@@ -289,4 +289,35 @@ __device__ __forceinline__ ulonglong2 view_substr(const ulonglong2& v, long long
   return r;
 }
 
+// character_length(view): the bytes that are not UTF-8 continuation bytes (10xxxxxx), which for valid UTF-8 is DataFusion's
+// chars().count().  A zero byte is never a continuation byte, so words loaded only in part are zero-extended.
+__device__ __forceinline__ uint32_t utf8_cont_bytes(uint64_t w) { return (uint32_t)__popcll(w & ~(w << 1) & 0x8080808080808080ull); }
+__device__ __forceinline__ int32_t view_char_length(const ulonglong2& v) {
+  const uint32_t n = (uint32_t)v.x;
+  if (n <= 12) {       // inline: bytes 0-3 in the high half of x, 4-11 in y; whatever lies past byte n is masked off
+    const uint64_t hx = (v.x >> 32) & (n >= 4 ? 0xFFFFFFFFull : (1ull << (8 * n)) - 1);
+    const uint64_t hy = n >= 12 ? v.y : v.y & ((1ull << (8 * (n > 4 ? n - 4 : 0))) - 1);
+    return (int32_t)(n - utf8_cont_bytes(hx) - utf8_cont_bytes(hy));
+  }
+  // Long string: every load is naturally aligned and lies inside [p, p + n), since a batch pushed from a foreign device buffer
+  // may end exactly at its last string byte.  1-, 2- and 4-byte loads reach 8-byte alignment (n >= 13 keeps them inside), one
+  // 8-byte load reaches 16, 16-byte loads cover the middle and 8-, 4-, 2- and 1-byte loads the tail.
+  const uint8_t* p = reinterpret_cast<const uint8_t*>(v.y);
+  const uint8_t* const e = p + n;
+  uint32_t c = 0;
+  if (reinterpret_cast<unsigned long long>(p) & 1) { c += utf8_cont_bytes(__ldg(p)); p += 1; }
+  if (reinterpret_cast<unsigned long long>(p) & 2) { c += utf8_cont_bytes(__ldg(reinterpret_cast<const unsigned short*>(p))); p += 2; }
+  if (reinterpret_cast<unsigned long long>(p) & 4) { c += utf8_cont_bytes(__ldg(reinterpret_cast<const unsigned int*>(p))); p += 4; }
+  if ((reinterpret_cast<unsigned long long>(p) & 8) && p + 8 <= e) { c += utf8_cont_bytes(__ldg(reinterpret_cast<const unsigned long long*>(p))); p += 8; }
+  for (; p + 16 <= e; p += 16) {
+    const ulonglong2 w = __ldg(reinterpret_cast<const ulonglong2*>(p));
+    c += utf8_cont_bytes(w.x) + utf8_cont_bytes(w.y);
+  }
+  if (p + 8 <= e) { c += utf8_cont_bytes(__ldg(reinterpret_cast<const unsigned long long*>(p))); p += 8; }
+  if (p + 4 <= e) { c += utf8_cont_bytes(__ldg(reinterpret_cast<const unsigned int*>(p))); p += 4; }
+  if (p + 2 <= e) { c += utf8_cont_bytes(__ldg(reinterpret_cast<const unsigned short*>(p))); p += 2; }
+  if (p < e) c += utf8_cont_bytes(__ldg(p));
+  return (int32_t)(n - c);
+}
+
 }  // namespace sg

@@ -1,7 +1,7 @@
 // expr.hpp -- physical expressions: parsing from the JSON spec and DataFusion/arrow-rs type rules.
 //
 // Mirrors what Sail hands DataFusion after planning: BinaryExpr / Literal / Column / CastExpr /
-// CaseExpr / InListExpr / LikeExpr / NotExpr / IsNull / ScalarFunction(date_part, substr)
+// CaseExpr / InListExpr / LikeExpr / NotExpr / IsNull / ScalarFunction(date_part, date_trunc, substr, character_length)
 // (crates/sail-plan/src/function/scalar/math.rs:48-181,580-583; predicate.rs:103-125).
 // Result types follow arrow-arith 58 (SURVEY.md Appendix A).
 #pragma once
@@ -16,7 +16,7 @@ struct Expr;
 using ExprPtr = std::shared_ptr<Expr>;
 
 struct Expr {
-  enum Kind { Col, Lit, Bin, Not, Neg, IsNull, IsNotNull, Cast, Case, Like, DatePart, Substr, DateTrunc } kind = Col;
+  enum Kind { Col, Lit, Bin, Not, Neg, IsNull, IsNotNull, Cast, Case, Like, DatePart, Substr, DateTrunc, CharLength } kind = Col;
   DataType type;
   bool nullable = false;
   // Col
@@ -290,6 +290,14 @@ inline ExprPtr parse_expr(const Json& j, const Schema& in) {
       SG_CHECK(!(ln && !ln->is_null()) || e->sub_len >= 0, SAILGPU_ERR_INVALID, "substr with a negative length");
       e->op = "substr:" + std::to_string(e->sub_start) + ":" + std::to_string(e->sub_len);
       e->type = e->args[0]->type; e->nullable = e->args[0]->nullable;
+      return e;
+    }
+    if (fn == "character_length") {      // characters of a Utf8 / Utf8View string as Int32, DataFusion's type for both
+      e->kind = Expr::CharLength;
+      SG_CHECK(j.at("args").a.size() == 1, SAILGPU_ERR_INVALID, "character_length takes one argument");
+      e->args = {parse_expr(j.at("args").a[0], in)};
+      SG_CHECK(e->args[0]->type.is_string(), SAILGPU_ERR_INVALID, "character_length needs a string operand");
+      e->type = T(TypeId::Int32); e->nullable = e->args[0]->nullable;
       return e;
     }
     fail(SAILGPU_ERR_UNSUPPORTED, "scalar function '" + fn + "' is not implemented on the GPU path");

@@ -204,6 +204,7 @@ struct Emitter {
       case OP_SUBSTR:
         def(I.dst, K_V16, "(inb ? view_substr(" + operand(I.a, K_V16, I.sa) + ", " + std::to_string((long long)I.imm0) + "ll, " + std::to_string((long long)I.imm1) + "ll) : mkv16(0ull, 0ull))");
         break;
+      case OP_CHAR_LEN: def(I.dst, K_I32, "(inb ? view_char_length(" + operand(I.a, K_V16, I.sa) + ") : 0)"); break;
       case OP_PROBE: {       // dst = matched (B), a = build row id (I64), c = rows still active (B) or none
         const JitInfo::Probe& pr = J.probes.at(I.aux);
         const std::string key = pr.key0.width == 8 ? "(uint64_t)" + operand(pr.key0.slot, K_I64, pr.key0.stride)

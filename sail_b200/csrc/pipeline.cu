@@ -282,6 +282,17 @@ __device__ __noinline__ void vm_like(const VmInst& I, const TileCtx& c) {
   }
 }
 
+// OP_CHAR_LEN: out of line like the other string instructions
+template <int RPT>
+__device__ __noinline__ void vm_char_len(const VmInst& I, const TileCtx& c) {
+  const uint8_t* pa = c.arena + eff(c, I.a);
+  uint8_t* pd = c.arena + eff(c, I.dst);
+  for (int k = 0; k < RPT; ++k) {
+    const int r = threadIdx.x + k * NT;
+    sts<int32_t>(pd + r * 4, r < c.nrows ? view_char_length(*reinterpret_cast<const ulonglong2*>(pa + r * I.sa)) : 0);
+  }
+}
+
 // OP_TS_PART / OP_TS_TRUNC: out of line, so that the main VM switch keeps its registers.  The unit is chosen once per
 // instruction, outside the row loop, so each loop divides by constants only.
 template <int RPT, int64_t UPS, bool TRUNC>
@@ -681,6 +692,7 @@ __device__ __forceinline__ void vm_exec(const VmInst* prog, int n_inst, const Ti
         }
         break;
       }
+      case OP_CHAR_LEN: vm_char_len<RPT>(I, c); break;
       case OP_TS_PART: vm_ts<RPT, false>(I, c); break;
       case OP_TS_TRUNC: vm_ts<RPT, true>(I, c); break;
       case OP_PROBE: vm_probe<RPT>(aux->probe[I.aux], c, I.c); break;

@@ -33,7 +33,7 @@ inline bool timing_enabled() { static const bool on = getenv("SAILGPU_TIMING") !
 inline void dump_pipeline(const CompiledPipeline& cp) {
   static const char* names[] = {"NOP", "UNPACK_BITS", "CONST", "MOV", "CVT", "ADD", "SUB", "MUL", "DIV", "REM", "NEG", "MULW", "MUL128_64", "DIVROUND",
                                 "EQ", "NE", "LT", "LE", "GT", "GE", "AND", "OR", "NOT", "ANDNOT", "SELECT", "STR_EQ_LONG", "STR_LIKE", "DATE_PART", "PROBE", "GATHER", "SUBSTR",
-                                "TS_PART", "TS_TRUNC", "MUL_POW10_CHK"};
+                                "TS_PART", "TS_TRUNC", "MUL_POW10_CHK", "CHAR_LEN"};
   static const char* sinks[] = {"STORE", "COMPACT", "AGG", "BUILD", "PARTITION"};
   fprintf(stderr, "[sailgpu pipeline] sink=%s rows/thread=%d stages=%d smem=%zu B (temps %u, stage %u, hot %u) inputs=%zu outs=%zu%s\n",
           cp.sink >= 0 && cp.sink < 5 ? sinks[cp.sink] : "?", cp.rpt, cp.n_stages, cp.smem_bytes, cp.temps_bytes, cp.stage_bytes, cp.hot_bytes,

@@ -57,6 +57,7 @@ enum VmBase : uint16_t {
   OP_TS_TRUNC,      // dst(I64) <- timestamp a(I64) truncated to part (aux) in the zone; imm0 / imm1 as OP_TS_PART
   OP_MUL_POW10_CHK, // dst(I128) <- a(I128) * imm (a power of ten); ERR_OVERFLOW when a row of c (rows evaluated, or NO_SLOT
                     //   for all) leaves i128: the decimal division rescale that can overflow
+  OP_CHAR_LEN,      // dst(I32) <- character_length(view a): UTF-8 characters
   OP_COUNT_
 };
 // OP_TS_PART / OP_TS_TRUNC parts.  TS_SECOND: the part is the microsecond within the minute, the truncation the whole second;

@@ -148,6 +148,10 @@ def substr(e, start: int, length: int | None = None):
     return {"fn": "substr", "args": [e], "start": start, "length": length}
 
 
+def char_length(e):
+    return {"fn": "character_length", "args": [e]}
+
+
 def sort(child: Node, keys: list, fetch=None) -> Node:
     """keys: (column name, asc) -- Spark default null ordering: ASC NULLS FIRST / DESC NULLS LAST"""
     ks = [{"expr": resolve(col(k), child.names), "asc": asc, "nulls_first": asc} for k, asc in keys]

@@ -92,9 +92,14 @@ pub fn expr(e: &Arc<dyn PhysicalExpr>) -> Option<Value> {
         return Some(json!({"in": expr(i.expr())?, "set": set?, "negated": i.negated()}));
     }
     if let Some(f) = any.downcast_ref::<ScalarFunctionExpr>() {
+        let name = f.name().to_lowercase();
+        if name == "character_length" {
+            // Spark's length / char_length / character_length (Utf8 or Utf8View -> Int32)
+            let [arg] = f.args() else { return None };
+            return Some(json!({"fn": name, "args": [expr(arg)?]}));
+        }
         // date_part / date_trunc with a literal part: DataFusion's simplifier has already folded Sail's part conversion
         // (`CASE WHEN 'minute' ILIKE ..`) to a literal, as the Partial aggregate's group keys in the ClickBench snapshot show
-        let name = f.name().to_lowercase();
         if name != "date_part" && name != "date_trunc" { return None; }
         let [part, arg] = f.args() else { return None };
         let part = match part.as_any().downcast_ref::<Literal>()?.value() {
