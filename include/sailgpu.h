@@ -318,11 +318,8 @@ SAILGPU_API void sailgpu_host_free(sailgpu_ctx* ctx, void* p);
 /* Environment (read by the library; all optional, none changes results):
  *   SAILGPU_JIT=0                 interpret every pipeline;  SAILGPU_JIT_MIN_ROWS=n  rows a pipeline must have seen before it is specialised
  *   SAILGPU_JIT_CACHE=dir         where cubins are kept;  SAILGPU_JIT_VERBOSE / _STRICT / _DUMP  diagnostics of the specialiser
- *   SAILGPU_JIT_PROBE=1           specialise hash-join probe pipelines too (slower than the interpreter as tuned: off)
- *   SAILGPU_DIRECT_KEY=1          direct-key protocol for single-word group keys (slower end to end as tuned: off)
- *   SAILGPU_NO_JOIN_SWAP=1        never exchange the roles of a join's inputs;  SAILGPU_TOPK_MIN_ROWS=n  TopK selection threshold
+ *   SAILGPU_TOPK_MIN_ROWS=n       TopK selection threshold;  SAILGPU_AGG_MIN_CAPACITY=n  first group-table size
  *   SAILGPU_PACK_THREADS=n        packer threads of the host ingest (default: the CPUs the cgroup grants, at most 32)
- *   SAILGPU_H2D_PACK=0 / SAILGPU_PACK_ONE_PASS=0 / SAILGPU_PACK_PIECE_ROWS=n / SAILGPU_PACK_NUMA=0 / SAILGPU_PACK_DRY=1   ingest A/B knobs
- *   SAILGPU_PACKED_EXCHANGE=1     small exchange messages as one buffer per peer;  SAILGPU_AGG_MIN_CAPACITY=n  first group-table size */
+ *   SAILGPU_H2D_PACK=0 / SAILGPU_PACK_PIECE_ROWS=n / SAILGPU_PACK_NUMA=0   ingest A/B knobs */
 
 #endif /* SAILGPU_H */

@@ -452,16 +452,6 @@ void PipelineCompiler::finish_aggregate(CompiledPipeline& out, const StageSpec& 
   if (cas128 && ((2 + A.key_words + words) & 1)) ++words;
   A.acc_words = words;
   A.entry_words = (uint32_t)(2 + A.key_words + A.acc_words);
-  // thread-private layout: [seen?][one word per accumulator; two for 128-bit min/max]
-  bool any_seen = false;
-  for (int j = 0; j < A.n_accs; ++j) any_seen |= A.accs[j].track_seen != 0;
-  A.priv_seen = any_seen ? 1 : 0;
-  int pw = A.priv_seen;
-  for (int j = 0; j < A.n_accs; ++j) {
-    A.accs[j].pword = (uint16_t)pw;
-    pw += (A.accs[j].op == ACC_MIN_I128 || A.accs[j].op == ACC_MAX_I128) ? 2 : 1;
-  }
-  A.priv_words = pw;
   // integer fast path: every accumulator is a count or an integer/decimal sum without validity-dependent
   // NULL results, and few enough to live in registers
   {
@@ -578,7 +568,6 @@ void PipelineCompiler::finalize(CompiledPipeline& out, Ctx* ctx, int hot_wanted)
     J.agg.hot_groups = best_hot;
     if (out.cold_variant) { J.agg.cold_only = 1; J.agg.reg_path = 0; }
     if (best_hot < REG_GROUPS) J.agg.reg_path = 0;
-    for (ProbeParams* pp : probe_params) J.probes.push_back({pp->n_keys, pp->keys[0]});
     J.valid = true;
   }
   auto off = [&](uint32_t id) -> uint32_t { return id == NO_SLOT ? NO_SLOT : slots_.at(id).offset; };

@@ -58,8 +58,6 @@ struct JitInfo {
   AggParams agg{};                   // keys / accs carry slot ids
   bool small_acc[MAX_ACCS] = {};
   std::vector<KeyDesc> keys;
-  struct Probe { int n_keys; KeyDesc key0; };   // join probes of the pipeline: first key with slot IDS (single-key probes are specialised)
-  std::vector<Probe> probes;
 };
 struct JitKernel;
 

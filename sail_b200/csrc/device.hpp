@@ -130,9 +130,8 @@ inline BufPtr dev_alloc(Ctx* ctx, size_t bytes) {
   b->ctx = ctx;
   b->bytes = bytes;
   const size_t padded = ((bytes + 255) & ~(size_t)255) + 256;   // room for 16-byte over-reads of tails
-  static const bool no_cache = getenv("SAILGPU_NO_ALLOC_CACHE") != nullptr;
-  const size_t cls = no_cache ? 0 : Ctx::size_class(padded);
-  if (cls) {
+  const size_t cls = Ctx::size_class(padded);
+  {
     std::lock_guard<std::mutex> g(ctx->cache_mu);
     auto it = ctx->cache.find(cls);
     if (it != ctx->cache.end() && !it->second.empty()) {
@@ -140,8 +139,8 @@ inline BufPtr dev_alloc(Ctx* ctx, size_t bytes) {
       return b;
     }
   }
-  cudaError_t e = cudaMallocAsync(&b->ptr, cls ? cls : padded, ctx->stream);
-  if (e == cudaErrorMemoryAllocation && cls) {       // out of HBM with blocks parked in the cache: give them back and retry
+  cudaError_t e = cudaMallocAsync(&b->ptr, cls, ctx->stream);
+  if (e == cudaErrorMemoryAllocation) {       // out of HBM with blocks parked in the cache: give them back and retry
     cudaGetLastError();
     {
       std::lock_guard<std::mutex> g(ctx->cache_mu);

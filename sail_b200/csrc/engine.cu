@@ -116,7 +116,6 @@ void check_device_error(Ctx* ctx, uint32_t* dev_flag) {
 struct AggTable {
   BufPtr table, state, occ;
   uint64_t capacity = 0;
-  bool direct = false;        // direct-key protocol (vm.h AggParams::direct_key): `occ` is built on demand
 };
 
 struct PipelineOp : Op {
@@ -336,25 +335,6 @@ struct PipelineOp : Op {
     A.occ = static_cast<uint32_t*>(tab.occ->ptr);
     A.capacity_mask = tab.capacity - 1;
     A.n_groups = run.scal.n_groups();
-    A.direct_key = tab.direct ? 1 : 0;
-  }
-  // One never-null 8-byte key word: the table CAN take the direct-key protocol.  Opt-in (SAILGPU_DIRECT_KEY=1): on GROUP BY
-  // l_orderkey over SF10 (60 M rows -> 15 M groups) the insert kernel itself did not get faster without the fence and the counter
-  // round trip (it is bound by the per-row accumulator atomics that need their old value for the 128-bit carry), while
-  // initialising and scanning every ENTRY of the 64 M-slot table costs more than the 4-byte state words of the general protocol
-  // (as tuned; not re-measured on H100).
-  static bool direct_eligible(const AggParams& A) {
-    const char* e = getenv("SAILGPU_DIRECT_KEY");
-    return A.n_keys == 1 && A.key_words == 1 && !A.has_null_word && e && *e && atoi(e) != 0;
-  }
-  // direct-key tables keep no list of occupied entries while they are filled: build it (extraction / re-hash / migration read it)
-  void build_occ(const AggTable& t, const AggParams& layout) {
-    if (!t.direct) return;
-    AggParams A = layout;
-    A.table = static_cast<uint8_t*>(t.table->ptr); A.occ = static_cast<uint32_t*>(t.occ->ptr); A.capacity_mask = t.capacity - 1;
-    BufPtr counter = dev_alloc_zero(ctx, 8);
-    SG_CUDA(launch_agg_build_occ(A, static_cast<unsigned long long*>(counter->ptr), ctx->stream));
-    m.kernel_launches++;
   }
 
   // (re)allocates the table with `cap` slots and moves the `groups` existing entries over
@@ -362,13 +342,10 @@ struct PipelineOp : Op {
     SG_CHECK(cap <= MAX_CAPACITY, SAILGPU_ERR_UNSUPPORTED, "aggregate needs more than 2^28 group slots");
     AggTable old = tab;
     tab.capacity = cap;
-    tab.direct = direct_eligible(A0);
-    tab.table = dev_alloc(ctx, (size_t)(cap + 1) * A0.entry_words * 8);
-    tab.state = tab.direct ? dev_alloc(ctx, 4) : dev_alloc_zero(ctx, (size_t)cap * 4);
-    tab.occ = dev_alloc(ctx, (size_t)(cap + 1) * 4);
-    if (tab.direct) { run.ensure_scratch(); AggParams A = A0; fill_table(A); SG_CUDA(launch_agg_init_direct(A, ctx->stream)); m.kernel_launches++; }
+    tab.table = dev_alloc(ctx, (size_t)cap * A0.entry_words * 8);
+    tab.state = dev_alloc_zero(ctx, (size_t)cap * 4);
+    tab.occ = dev_alloc(ctx, (size_t)cap * 4);
     if (old.capacity && groups) {
-      build_occ(old, A0);
       AggParams A = A0;
       fill_table(A);
       SG_CUDA(cudaMemsetAsync(run.scal.n_groups(), 0, 8, ctx->stream));
@@ -462,15 +439,12 @@ struct PipelineOp : Op {
     }
     const uint64_t groups = current_groups();
     AggTable old = tab;
-    build_occ(old, O);
-    tab.direct = direct_eligible(N);
-    tab.table = dev_alloc(ctx, (size_t)(tab.capacity + 1) * N.entry_words * 8);
-    tab.state = tab.direct ? dev_alloc(ctx, 4) : dev_alloc_zero(ctx, (size_t)tab.capacity * 4);
-    tab.occ = dev_alloc(ctx, (size_t)(tab.capacity + 1) * 4);
+    tab.table = dev_alloc(ctx, (size_t)tab.capacity * N.entry_words * 8);
+    tab.state = dev_alloc_zero(ctx, (size_t)tab.capacity * 4);
+    tab.occ = dev_alloc(ctx, (size_t)tab.capacity * 4);
     run.ensure_scratch();
     AggParams A = N;
     fill_table(A);
-    if (tab.direct) { SG_CUDA(launch_agg_init_direct(A, ctx->stream)); m.kernel_launches++; }
     SG_CUDA(cudaMemsetAsync(run.scal.n_groups(), 0, 8, ctx->stream));
     SG_CUDA(launch_agg_migrate(A, M, static_cast<const uint8_t*>(old.table->ptr), static_cast<const uint32_t*>(old.occ->ptr), groups, run.scal.error(), ctx->stream));
     m.kernel_launches++;
@@ -562,7 +536,7 @@ struct PipelineOp : Op {
         }
       }
       if (cap > tab.capacity) alloc_table(inflight.front().cp->agg, cap, groups);
-      if (!use_cold && groups > CARD_MANY_GROUPS && getenv("SAILGPU_NO_COLD") == nullptr) {
+      if (!use_cold && groups > CARD_MANY_GROUPS) {
         auto cold = run.compiled_for(*inflight.front().batch, true);
         if (cold->agg.entry_words == inflight.front().cp->agg.entry_words) use_cold = true;     // later batches start on the many-groups variant
       }
@@ -645,7 +619,6 @@ struct PipelineOp : Op {
       out->cols.push_back(c);
     }
     if (!synth && rows > 0) {
-      build_occ(tab, A0);
       AggParams A = A0;
       fill_table(A);
       SG_CUDA(launch_agg_extract(A, X, groups, run.scal.error(), ctx->stream));
@@ -712,8 +685,7 @@ struct PipelineOp : Op {
   void spill(uint64_t groups) {
     Trace tr(ctx, "agg.spill");
     BatchPtr rows = extract_rows(*agg_cp, state_outs(*agg_cp), groups);
-    if (tab.direct) { AggParams A = agg_cp->agg; fill_table(A); SG_CUDA(launch_agg_init_direct(A, ctx->stream)); m.kernel_launches++; }
-    else SG_CUDA(cudaMemsetAsync(tab.state->ptr, 0, (size_t)tab.capacity * 4, ctx->stream));
+    SG_CUDA(cudaMemsetAsync(tab.state->ptr, 0, (size_t)tab.capacity * 4, ctx->stream));
     SG_CUDA(cudaMemsetAsync(run.scal.n_groups(), 0, 8, ctx->stream));
     known_groups = -1;
     m.agg_spills++;

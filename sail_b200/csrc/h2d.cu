@@ -28,8 +28,6 @@ static int64_t piece_rows() {      // read per batch: A/B measurements in one pr
   const int64_t r = e && *e ? atoll(e) : MAX_PIECE_ROWS;
   return std::max<int64_t>(1024, std::min<int64_t>(MAX_PIECE_ROWS, r / 1024 * 1024));
 }
-// SAILGPU_PACK_DRY=1 (measurements only): pieces are packed but neither copied nor expanded -- the host side of the ingest alone
-static bool pack_dry() { const char* e = getenv("SAILGPU_PACK_DRY"); return e && *e && atoi(e) != 0; }
 
 enum Enc : int { ENC_RAW = 0, ENC_INT = 1, ENC_VIEW = 2 };
 
@@ -109,23 +107,17 @@ static inline bool fits(long long mn, long long mx, long long base, int w) {
   const unsigned long long top = (unsigned long long)mx - (unsigned long long)base;
   return w >= 8 || top < (w == 4 ? (1ull << 32) : (1ull << (8 * w)));
 }
-static bool one_pass() { const char* e = getenv("SAILGPU_PACK_ONE_PASS"); return !(e && *e && atoi(e) == 0); }      // read per piece (A/B measurements)
 
 static Packed pack_piece(const HostStager::Item& it, uint8_t* out, bool narrow) {
   const int64_t n = it.n;
   if (narrow && n > 0 && it.kind == HostCol::Dec128) {
     const int64_t* p = reinterpret_cast<const int64_t*>(it.src);
     int64_t mn, mx; uint64_t bad = 0;
-    bool scanned = false;
-    if (one_pass()) {
-      const Guess g = guess_range(p, n, 2, 4);
-      if (g.ok) {
-        sg_packchk_dec128(out, p, n, g.base, g.w, &mn, &mx, &bad);
-        if (!bad && fits(mn, mx, g.base, g.w)) return {ENC_INT, (size_t)n * g.w, g.base, g.w};
-        scanned = true;
-      }
-    }
-    if (!scanned) sg_scan_dec128(p, n, &mn, &mx, &bad);
+    const Guess g = guess_range(p, n, 2, 4);
+    if (g.ok) {
+      sg_packchk_dec128(out, p, n, g.base, g.w, &mn, &mx, &bad);
+      if (!bad && fits(mn, mx, g.base, g.w)) return {ENC_INT, (size_t)n * g.w, g.base, g.w};
+    } else sg_scan_dec128(p, n, &mn, &mx, &bad);
     if (!bad) {
       const int w = width_for((unsigned long long)mx - (unsigned long long)mn);
       sg_pack_i64(out, p, 2, n, mn, w);
@@ -134,47 +126,35 @@ static Packed pack_piece(const HostStager::Item& it, uint8_t* out, bool narrow) 
   } else if (narrow && n > 0 && it.kind == HostCol::Int64) {
     const int64_t* p = reinterpret_cast<const int64_t*>(it.src);
     int64_t mn, mx;
-    bool scanned = false;
-    if (one_pass()) {
-      const Guess g = guess_range(p, n, 1, 4);
-      if (g.ok) {
-        sg_packchk_i64(out, p, n, g.base, g.w, &mn, &mx);
-        if (fits(mn, mx, g.base, g.w)) return {ENC_INT, (size_t)n * g.w, g.base, g.w};
-        scanned = true;
-      }
-    }
-    if (!scanned) sg_scan_i64(p, n, &mn, &mx);
+    const Guess g = guess_range(p, n, 1, 4);
+    if (g.ok) {
+      sg_packchk_i64(out, p, n, g.base, g.w, &mn, &mx);
+      if (fits(mn, mx, g.base, g.w)) return {ENC_INT, (size_t)n * g.w, g.base, g.w};
+    } else sg_scan_i64(p, n, &mn, &mx);
     const int w = width_for((unsigned long long)mx - (unsigned long long)mn);
     if (w < 8) { sg_pack_i64(out, p, 1, n, mn, w); return {ENC_INT, (size_t)n * w, mn, w}; }
   } else if (narrow && n > 0 && it.kind == HostCol::Int32) {
     const int32_t* p = reinterpret_cast<const int32_t*>(it.src);
     int32_t mn, mx;
-    bool scanned = false;
-    if (one_pass()) {
-      const Guess g = guess_range(p, n, 1, 2);
-      if (g.ok && g.base >= INT32_MIN) {
-        sg_packchk_i32(out, p, n, (int32_t)g.base, g.w, &mn, &mx);
-        if (fits(mn, mx, g.base, g.w)) return {ENC_INT, (size_t)n * g.w, g.base, g.w};
-        scanned = true;
-      }
-    }
-    if (!scanned) sg_scan_i32(p, n, &mn, &mx);
+    const Guess g = guess_range(p, n, 1, 2);
+    if (g.ok && g.base >= INT32_MIN) {
+      sg_packchk_i32(out, p, n, (int32_t)g.base, g.w, &mn, &mx);
+      if (fits(mn, mx, g.base, g.w)) return {ENC_INT, (size_t)n * g.w, g.base, g.w};
+    } else sg_scan_i32(p, n, &mn, &mx);
     const int w = width_for((unsigned long long)((long long)mx - (long long)mn));
     if (w < 4) { sg_pack_i32(out, p, n, mn, w); return {ENC_INT, (size_t)n * w, (long long)mn, w}; }
   } else if (narrow && n > 0 && it.kind == HostCol::View16) {
     const uint32_t* lens = reinterpret_cast<const uint32_t*>(it.src);
     uint32_t L = 13;
-    if (one_pass()) {
-      const int64_t step = std::max<int64_t>(1, n / N_SAMPLES);
-      for (int64_t i = 0; i < n; i += step) __builtin_prefetch(lens + 4 * i);
-      uint32_t Ls = 0;
-      for (int64_t i = 0; i < n; i += step) Ls = std::max(Ls, lens[4 * i]);
-      if (Ls <= 12) {
-        L = sg_packchk_views(out, it.src, n, Ls);
-        if (L <= Ls) return {ENC_VIEW, (size_t)(1 + Ls) * (size_t)n, 0, (int)Ls};
-      }
+    const int64_t step = std::max<int64_t>(1, n / N_SAMPLES);
+    for (int64_t i = 0; i < n; i += step) __builtin_prefetch(lens + 4 * i);
+    uint32_t Ls = 0;
+    for (int64_t i = 0; i < n; i += step) Ls = std::max(Ls, lens[4 * i]);
+    if (Ls <= 12) {
+      L = sg_packchk_views(out, it.src, n, Ls);
+      if (L <= Ls) return {ENC_VIEW, (size_t)(1 + Ls) * (size_t)n, 0, (int)Ls};
     }
-    if (L > 12) L = sg_scan_view_maxlen(lens, n);      // (a rejected one-pass attempt left the true maximum in L)
+    if (L > 12) L = sg_scan_view_maxlen(lens, n);      // (a rejected guess left the true maximum in L)
     if (L <= 12) { sg_pack_views(out, it.src, n, L); return {ENC_VIEW, (size_t)(1 + L) * (size_t)n, 0, (int)L}; }
   }
   const size_t bytes = (size_t)n * (size_t)it.width;
@@ -246,7 +226,6 @@ struct PackPool {
     Slot& s = w.slots[(size_t)(w.turn++ & 1)];
     if (s.used && cudaEventSynchronize(s.free_ev) != cudaSuccess) throw std::runtime_error("staging slot event");
     const Packed pk = pack_piece(it, s.host, narrow);
-    if (pack_dry()) { ctx->h2d_bytes += pk.bytes; return; }
     cudaError_t e;
     if (pk.enc == ENC_RAW) {
       e = cudaMemcpyAsync(it.dst, s.host, pk.bytes, cudaMemcpyHostToDevice, w.stream);

@@ -205,27 +205,6 @@ struct Emitter {
         def(I.dst, K_V16, "(inb ? view_substr(" + operand(I.a, K_V16, I.sa) + ", " + std::to_string((long long)I.imm0) + "ll, " + std::to_string((long long)I.imm1) + "ll) : mkv16(0ull, 0ull))");
         break;
       case OP_CHAR_LEN: def(I.dst, K_I32, "(inb ? view_char_length(" + operand(I.a, K_V16, I.sa) + ") : 0)"); break;
-      case OP_PROBE: {       // dst = matched (B), a = build row id (I64), c = rows still active (B) or none
-        const JitInfo::Probe& pr = J.probes.at(I.aux);
-        const std::string key = pr.key0.width == 8 ? "(uint64_t)" + operand(pr.key0.slot, K_I64, pr.key0.stride)
-                                                   : "(uint64_t)(uint32_t)" + operand(pr.key0.slot, K_I32, pr.key0.stride);
-        std::string act = "inb";
-        if (I.c != NO_SLOT) act += " && " + operand(I.c, K_B, 1);
-        if (pr.key0.valid_slot != NO_SLOT) act += " && " + operand(pr.key0.valid_slot, K_B, 1);      // NULL keys match nothing
-        def(I.a, K_I64, "jit_probe_narrow(K.aux[0].probe[" + std::to_string(I.aux) + "], " + key + ", " + std::to_string((int)pr.key0.width) + ", " + act + ")");
-        def(I.dst, K_B, "(t" + std::to_string(I.a) + " >= 0)");
-        break;
-      }
-      case OP_GATHER: {      // dst(kind) = build column [K.prog[..].imm1] at row id a (or zero); aux = element width
-        const std::string row = operand(I.a, K_I64, 8);
-        const std::string ptr = "K.prog[0][" + std::to_string(pc) + "].imm1";
-        if (kind == K_B) def(I.dst, K_B, "(jit_gather<uint8_t>(" + ptr + ", " + row + ") != 0)");
-        else {
-          if (kind_width(kind) != (int)I.aux) throw Unsupported{"gather width differs from the value kind"};
-          def(I.dst, kind, "jit_gather<" + T + ">(" + ptr + ", " + row + ")");
-        }
-        break;
-      }
       case OP_DATE_PART: def(I.dst, K_I32, "jit_date_part(" + operand(I.a, K_I32, I.sa) + ", " + std::to_string(I.aux) + ")"); break;
       case OP_TS_PART: case OP_TS_TRUNC: {   // unit and zone offset become constants: the divisions strength-reduce
         const std::string call = std::string(base == OP_TS_TRUNC ? "ts_trunc_u<" : "ts_part_u<") + std::to_string((long long)I.imm0) + "ll>(" +
@@ -431,17 +410,10 @@ bool jit_supported(const CompiledPipeline& cp, std::string* why) {
   if (!cp.jit.valid) return no("no specialiser snapshot");
   if (cp.sink != SINK_AGG && cp.sink != SINK_STORE && cp.sink != SINK_COMPACT) return no("sink is not aggregate / store / compact");
   if (cp.jit.inputs.empty()) return no("pipeline reads no column");
-  if (cp.n_probes > 0) {      // hash-join probe pipelines: one key of at most 8 bytes per probe (the PK-FK joins); store / compact sinks
-    // Opt-in (SAILGPU_JIT_PROBE=1): correct (the relational suite passes with it), but slower than the interpreter on
-    // orders x lineitem when it was tuned (not re-measured on H100): the interpreter's probe issues the first-slot loads of all rows of a thread
-    // before the dependent key loads, the generated code resolves one row at a time -- latency, not instructions, bounds a probe.
-    static const bool on = getenv("SAILGPU_JIT_PROBE") != nullptr && atoi(getenv("SAILGPU_JIT_PROBE")) != 0;
-    if (!on) return no("join probes run on the interpreter (SAILGPU_JIT_PROBE=1 specialises them)");
-    if (cp.sink == SINK_AGG) return no("aggregate fused behind a join probe");
-    if (cp.jit.outs.empty()) return no("probe that only marks build rows");
-    if ((int)cp.jit.probes.size() != cp.n_probes) return no("probe snapshot incomplete");
-    for (auto& pr : cp.jit.probes) if (pr.n_keys != 1 || (pr.key0.width != 4 && pr.key0.width != 8)) return no("join probe with several keys or a 16-byte key");
-  }
+  // a specialised probe that resolves one row at a time was slower on orders x lineitem when it was measured (not on H100):
+  // the interpreter issues the first-slot loads of all rows of a thread before the dependent key loads, and latency, not
+  // instructions, bounds a probe
+  if (cp.n_probes > 0) return no("join probes run on the interpreter");
   return true;
 }
 

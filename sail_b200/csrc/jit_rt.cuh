@@ -107,64 +107,10 @@ __device__ __forceinline__ uint64_t i128_lo(i128 v) { return (uint64_t)(u128)v; 
 __device__ __forceinline__ uint64_t i128_hi(i128 v) { return (uint64_t)((u128)v >> 64); }
 
 // ================================================================================================
-// hash-join probe with one key of at most 8 bytes (pipeline.cu::vm_probe_narrow; table slot = {hash | 1, build row + 1})
-// ================================================================================================
-__device__ __forceinline__ int64_t jit_probe_narrow(const ProbeParams& P, uint64_t key, int width, bool act) {
-  if (!act) return -1;
-  const uint64_t h = mix64(0x243F6A8885A308D3ull ^ key);
-  const uint64_t tag = h | 1ull;
-  const uint8_t* bcol = P.build_keys[0];
-  const int bstride = P.build_stride[0];
-  uint64_t idx = (h >> 1) & P.capacity_mask;
-  int64_t row = -1;
-  for (;;) {
-    const ulonglong2 cur = *reinterpret_cast<const ulonglong2*>(P.table + idx * 16);
-    if (cur.x == 0) break;
-    if (cur.x == tag && load_key_word(bcol + ((int64_t)cur.y - 1) * bstride, width) == key) { row = (int64_t)cur.y - 1; break; }
-    idx = (idx + 1) & P.capacity_mask;
-  }
-  if (row >= 0 && P.visited) P.visited[row] = 1;
-  return row;
-}
-template <class T>
-__device__ __forceinline__ T jit_gather(uint64_t base, int64_t row) {
-  if (row < 0) return T{};
-  return *reinterpret_cast<const T*>(base + (uint64_t)row * sizeof(T));
-}
-
-// ================================================================================================
 // global group table (layout and protocol of pipeline.cu::agg_find_or_insert, constants from G)
 // ================================================================================================
 template <class G>
 __device__ __forceinline__ uint64_t* jit_find_or_insert(const AggParams& A, const typename G::Key& kw, uint64_t h, uint32_t* err) {
-  if constexpr (G::KEY_WORDS == 1) {
-    if (A.direct_key) {          // direct-key protocol (vm.h): one CAS on the key word, no fence, no state word
-      const unsigned long long k = kw.w[0];
-      if (k == DIRECT_EMPTY_KEY) {
-        uint64_t* e = reinterpret_cast<uint64_t*>(A.table) + (A.capacity_mask + 1) * G::ENTRY_WORDS;
-        if (*reinterpret_cast<volatile unsigned long long*>(e) == 0ull && atomicCAS(reinterpret_cast<unsigned long long*>(e), 0ull, h | 1ull) == 0ull) atomicAdd(A.n_groups, 1ull);
-        return e;
-      }
-      uint64_t idx = h & A.capacity_mask;
-      for (uint64_t probes = 0; probes <= A.capacity_mask; ++probes) {
-        uint64_t* e = reinterpret_cast<uint64_t*>(A.table) + idx * G::ENTRY_WORDS;
-        unsigned long long cur = *reinterpret_cast<volatile unsigned long long*>(e + 2);
-        if (cur == DIRECT_EMPTY_KEY) {
-          cur = atomicCAS(reinterpret_cast<unsigned long long*>(e + 2), DIRECT_EMPTY_KEY, k);
-          if (cur == DIRECT_EMPTY_KEY) {
-            e[0] = h | 1ull;
-            const unsigned m = __activemask();
-            if ((int)(threadIdx.x & 31) == __ffs(m) - 1) atomicAdd(A.n_groups, (unsigned long long)__popc(m));
-            return e;
-          }
-        }
-        if (cur == k) return e;
-        idx = (idx + 1) & A.capacity_mask;
-      }
-      atomicOr(err, ERR_TABLE_FULL);
-      return nullptr;
-    }
-  }
   const uint32_t tag = (uint32_t)(h >> 34) << 2;
   uint64_t idx = h & A.capacity_mask;
   uint64_t probes = 0;

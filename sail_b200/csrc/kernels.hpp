@@ -42,8 +42,6 @@ struct AggMigrateMap {
   int16_t acc_src_word[MAX_ACCS];    // first word (inside the old accumulator area) of the accumulator a new one continues
   int8_t seen_src[MAX_ACCS];         // old accumulator index whose seen bit carries over; -1: every old contribution was valid (bit set); -2: not tracked
 };
-cudaError_t launch_agg_init_direct(const AggParams& A, cudaStream_t s);
-cudaError_t launch_agg_build_occ(const AggParams& A, unsigned long long* counter, cudaStream_t s);
 cudaError_t launch_agg_migrate(const AggParams& A_new, const AggMigrateMap& M, const uint8_t* old_table, const uint32_t* old_occ, uint64_t old_groups, uint32_t* err, cudaStream_t s);
 cudaError_t launch_pipeline(const KernelArgs& K, int rpt, int n_stages, size_t smem_bytes, int grid, int minb, cudaStream_t stream);
 int pipeline_max_ctas_per_sm(int rpt, int minb, size_t smem_bytes, int sink, bool cold);

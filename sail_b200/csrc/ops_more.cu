@@ -251,7 +251,7 @@ struct JoinOp : Op {
   // streamed side (INTEGRATION.md: the join reports maintains_input_order = false).
   bool no_swap = false;
   bool swap_applies(const DevBatch& b) const {
-    return !no_swap && dup && jt == "inner" && b.rows * 16 < build->rows && getenv("SAILGPU_NO_JOIN_SWAP") == nullptr;
+    return !no_swap && dup && jt == "inner" && b.rows * 16 < build->rows;
   }
   static void remap_cols(Json& j, int nb, int np) {
     if (j.kind == Json::Obj) {
@@ -658,7 +658,7 @@ std::unique_ptr<Op> make_join_op(Ctx* ctx, const Json& spec, const std::vector<S
   const Json* jtj = spec.find("join_type");
   const std::string jt = jtj ? jtj->as_str() : "inner";
   const Json* fj = spec.find("filter");
-  if ((jt == "left_semi" || jt == "left_anti") && !(fj && !fj->is_null()) && getenv("SAILGPU_NO_JOIN_SWAP") == nullptr) {
+  if ((jt == "left_semi" || jt == "left_anti") && !(fj && !fj->is_null())) {
     auto plain = make_plain_join_op(ctx, spec, inputs);     // plan-time validation + output schema
     auto op = std::make_unique<LazySemiJoinOp>();
     op->ctx = ctx; op->kind = "hash_join"; op->in_schemas = inputs; op->out_schema = plain->out_schema; op->spec = spec;
@@ -1713,13 +1713,6 @@ namespace sg { void set_ctx_error(const std::string& m); }
 #define NCCL_CALL(expr) do { int _r = (expr); if (_r != 0) sg::fail(SAILGPU_ERR_CUDA, std::string("NCCL error: ") + g_nccl.GetErrorString(_r) + " at " #expr); } while (0)
 
 namespace sg {
-// uploads the segment table and runs all copies in one launch; *keep holds the table until the stream has used it
-static cudaError_t launch_multi_copy(Ctx* ctx, const std::vector<CopySeg>& segs, BufPtr* keep) {
-  *keep = dev_alloc(ctx, segs.size() * sizeof(CopySeg));
-  cudaError_t e = cudaMemcpyAsync((*keep)->ptr, segs.data(), segs.size() * sizeof(CopySeg), cudaMemcpyHostToDevice, ctx->stream);   // pageable source: staged before return
-  if (e != cudaSuccess) return e;
-  return launch_multi_copy_raw(static_cast<const CopySeg*>((*keep)->ptr), (int)segs.size(), ctx->stream);
-}
 // all-to-all of world_size device batches over the context's communicator: parts[p] goes to rank p; returns everything
 // that was sent to this rank (rows of rank 0 first, then rank 1, ...).
 //
@@ -1827,10 +1820,7 @@ BatchPtr exchange_batches(Ctx* ctx, const Schema& schema, const std::vector<Batc
     if (t.id == TypeId::Bool) bbytes[ci] = datas[ci]; else col.data = datas[ci];
     out->cols.push_back(col);
   }
-  // Small messages can travel PACKED: all column buffers of one (source, destination) pair in one staging buffer, one
-  // ncclSend/ncclRecv per pair instead of 2-3 per column.  Both sides derive the same layout from the all-gathered table.
-  // Opt-in (SAILGPU_PACKED_EXCHANGE=1): at N=4 it did not pay when it was tuned (not re-measured on H100).
-  constexpr int64_t PACK_LIMIT = 1 << 20;
+  // bytes of the message `src` sends to `dst` as the exchange metrics count them: every buffer rounded up to 16 bytes
   auto a16 = [](int64_t v) { return (v + 15) & ~(int64_t)15; };
   auto msg_bytes = [&](int src, int dst) {
     const int64_t k = cnt(src, dst, 0);
@@ -1838,41 +1828,6 @@ BatchPtr exchange_batches(Ctx* ctx, const Schema& schema, const std::vector<Batc
     for (size_t ci = 0; ci < ncols; ++ci) tot += a16(k * width_of(ci)) + (vneed(dst, ci) ? a16(k) : 0) + a16(cnt(src, dst, 1 + ci));
     return k ? tot : 0;
   };
-  static const bool no_pack = getenv("SAILGPU_PACKED_EXCHANGE") == nullptr;
-  std::vector<CopySeg> pack_segs, unpack_segs;
-  std::vector<BufPtr> send_stage((size_t)W), recv_stage((size_t)W);
-  for (int peer = 0; peer < W; ++peer) {
-    const int64_t ks = parts[(size_t)peer]->rows, kr = cnt(peer, me, 0);
-    const int64_t sb = msg_bytes(me, peer), rb = msg_bytes(peer, me);
-    if (ks && !no_pack && sb <= PACK_LIMIT) {
-      send_stage[(size_t)peer] = dev_alloc(ctx, (size_t)sb);
-      uint8_t* base = static_cast<uint8_t*>(send_stage[(size_t)peer]->ptr);
-      int64_t off = 0;
-      for (size_t ci = 0; ci < ncols; ++ci) {
-        const SendCol& sd = sc[(size_t)peer][ci];
-        const int64_t db = ks * width_of(ci), hb = schema[ci].type.is_string() ? sd.heap_bytes : 0;
-        pack_segs.push_back({static_cast<const uint8_t*>(sd.data->ptr), base + off, (unsigned long long)db}); off += a16(db);
-        if (sd.validity_bytes) { pack_segs.push_back({static_cast<const uint8_t*>(sd.validity_bytes->ptr), base + off, (unsigned long long)ks}); off += a16(ks); }
-        if (hb) pack_segs.push_back({static_cast<const uint8_t*>(sd.heap->ptr), base + off, (unsigned long long)hb});
-        off += a16(hb);
-      }
-    }
-    if (kr && !no_pack && rb <= PACK_LIMIT) {
-      recv_stage[(size_t)peer] = dev_alloc(ctx, (size_t)rb);
-      const uint8_t* base = static_cast<const uint8_t*>(recv_stage[(size_t)peer]->ptr);
-      int64_t off = 0;
-      for (size_t ci = 0; ci < ncols; ++ci) {
-        const int w = width_of(ci);
-        const int64_t db = kr * w, hb = cnt(peer, me, 1 + ci);
-        unpack_segs.push_back({base + off, static_cast<uint8_t*>(datas[ci]->ptr) + row_off[(size_t)peer] * w, (unsigned long long)db}); off += a16(db);
-        if (vrecv[ci]) { unpack_segs.push_back({base + off, static_cast<uint8_t*>(vbytes[ci]->ptr) + row_off[(size_t)peer], (unsigned long long)kr}); off += a16(kr); }
-        if (hb) unpack_segs.push_back({base + off, static_cast<uint8_t*>(heaps[ci]->ptr) + heap_off[ci][(size_t)peer], (unsigned long long)hb});
-        off += a16(hb);
-      }
-    }
-  }
-  BufPtr seg_keep_a, seg_keep_b;
-  if (!pack_segs.empty()) SG_CUDA(launch_multi_copy(ctx, pack_segs, &seg_keep_a));
   // bytes that cross NVLink (everything except the segment this rank keeps) and the device time of the grouped send/recv
   {
     uint64_t sent = 0, recvd = 0;
@@ -1885,18 +1840,16 @@ BatchPtr exchange_batches(Ctx* ctx, const Schema& schema, const std::vector<Batc
   struct GroupGuard { bool open = true; ~GroupGuard() { if (open) g_nccl.GroupEnd(); } } group_guard;     // an error below must not leave the group open
   for (int peer = 0; peer < W; ++peer) {
     const int64_t ks = parts[(size_t)peer]->rows, kr = cnt(peer, me, 0);
-    if (ks && send_stage[(size_t)peer]) NCCL_CALL(g_nccl.Send(send_stage[(size_t)peer]->ptr, (size_t)msg_bytes(me, peer), NCCL_INT8, peer, ctx->nccl_comm, ctx->stream));
-    if (kr && recv_stage[(size_t)peer]) NCCL_CALL(g_nccl.Recv(recv_stage[(size_t)peer]->ptr, (size_t)msg_bytes(peer, me), NCCL_INT8, peer, ctx->nccl_comm, ctx->stream));
     for (size_t ci = 0; ci < ncols; ++ci) {
       const DataType& t = schema[ci].type;
       const int w = width_of(ci);
       const SendCol& sd = sc[(size_t)peer][ci];
-      if (ks && !send_stage[(size_t)peer]) {
+      if (ks) {
         NCCL_CALL(g_nccl.Send(sd.data->ptr, (size_t)ks * w, NCCL_INT8, peer, ctx->nccl_comm, ctx->stream));
         if (sd.validity_bytes) NCCL_CALL(g_nccl.Send(sd.validity_bytes->ptr, (size_t)ks, NCCL_INT8, peer, ctx->nccl_comm, ctx->stream));
         if (t.is_string() && sd.heap_bytes) NCCL_CALL(g_nccl.Send(sd.heap->ptr, (size_t)sd.heap_bytes, NCCL_INT8, peer, ctx->nccl_comm, ctx->stream));
       }
-      if (kr && !recv_stage[(size_t)peer]) {
+      if (kr) {
         NCCL_CALL(g_nccl.Recv(static_cast<uint8_t*>(datas[ci]->ptr) + row_off[(size_t)peer] * w, (size_t)kr * w, NCCL_INT8, peer, ctx->nccl_comm, ctx->stream));
         if (vrecv[ci]) NCCL_CALL(g_nccl.Recv(static_cast<uint8_t*>(vbytes[ci]->ptr) + row_off[(size_t)peer], (size_t)kr, NCCL_INT8, peer, ctx->nccl_comm, ctx->stream));
         const int64_t hb = cnt(peer, me, 1 + ci);
@@ -1907,7 +1860,6 @@ BatchPtr exchange_batches(Ctx* ctx, const Schema& schema, const std::vector<Batc
   group_guard.open = false;
   NCCL_CALL(g_nccl.GroupEnd());
   if (xe1) { SG_CUDA(cudaEventRecord(xe1, ctx->stream)); ctx->exch_events.emplace_back(xe0, xe1); }      // read when metrics are asked for
-  if (!unpack_segs.empty()) SG_CUDA(launch_multi_copy(ctx, unpack_segs, &seg_keep_b));
   // 4. post-process (no read-back): rebase string views per source segment, pack byte columns into Arrow bitmaps
   for (size_t ci = 0; ci < ncols; ++ci) {
     DevColumn& col = out->cols[ci];

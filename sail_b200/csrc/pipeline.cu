@@ -734,37 +734,9 @@ __device__ __forceinline__ void load_tile_generic(const PipelineParams& P, uint8
 // ================================================================================================
 
 
-// direct-key protocol (AggParams::direct_key): the key word itself is the slot's lock
-__device__ __forceinline__ uint64_t* agg_find_or_insert_direct(const AggParams& A, unsigned long long k, uint64_t h, uint32_t* err) {
-  if (k == DIRECT_EMPTY_KEY) {                       // the sentinel as a real key: the entry behind the table
-    uint64_t* e = reinterpret_cast<uint64_t*>(A.table) + (A.capacity_mask + 1) * A.entry_words;
-    if (*reinterpret_cast<volatile unsigned long long*>(e) == 0ull && atomicCAS(reinterpret_cast<unsigned long long*>(e), 0ull, h | 1ull) == 0ull) atomicAdd(A.n_groups, 1ull);
-    return e;
-  }
-  uint64_t idx = h & A.capacity_mask;
-  for (uint64_t probes = 0; probes <= A.capacity_mask; ++probes) {
-    uint64_t* e = reinterpret_cast<uint64_t*>(A.table) + idx * A.entry_words;
-    unsigned long long cur = *reinterpret_cast<volatile unsigned long long*>(e + 2);
-    if (cur == DIRECT_EMPTY_KEY) {
-      cur = atomicCAS(reinterpret_cast<unsigned long long*>(e + 2), DIRECT_EMPTY_KEY, k);
-      if (cur == DIRECT_EMPTY_KEY) {
-        e[0] = h | 1ull;
-        const unsigned m = __activemask();           // one counter update for the lanes that insert in the same step
-        if ((int)(threadIdx.x & 31) == __ffs(m) - 1) atomicAdd(A.n_groups, (unsigned long long)__popc(m));
-        return e;
-      }
-    }
-    if (cur == k) return e;
-    idx = (idx + 1) & A.capacity_mask;
-  }
-  atomicOr(err, ERR_TABLE_FULL);
-  return nullptr;
-}
-
 // state word: 0 = empty, else (tag30 << 2) | {1 = being written, 2 = ready}.  Carrying the tag in the
 // state lets a thread skip a slot that is being written for a different key without waiting on it.
 __device__ __forceinline__ uint64_t* agg_find_or_insert(const AggParams& A, const KeyRegs& key, uint64_t h, uint32_t* err) {
-  if (A.direct_key) return agg_find_or_insert_direct(A, key.w[0], h, err);
   const uint32_t tag = (uint32_t)(h >> 34) << 2;
   uint64_t idx = h & A.capacity_mask;
   uint64_t probes = 0;
@@ -1904,44 +1876,6 @@ __global__ void __launch_bounds__(NT, MINB) pipeline_kernel(const __grid_constan
 // ================================================================================================
 // helper kernels
 // ================================================================================================
-// direct-key tables: every entry starts as [0, 0, DIRECT_EMPTY_KEY, accumulator identities]
-__global__ void agg_init_direct_kernel(AggParams A, uint64_t n_entries) {
-  const uint64_t words = n_entries * A.entry_words;
-  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < words; i += (uint64_t)gridDim.x * blockDim.x) {
-    const uint32_t w = (uint32_t)(i % A.entry_words);
-    uint64_t v = 0;
-    if (w == 2) v = DIRECT_EMPTY_KEY;
-    else if (w >= 3) {
-      const int aw = (int)w - 3;
-      for (int j = 0; j < A.n_accs; ++j) {
-        const int nw = acc_words_of(A.accs[j].op);
-        if (aw >= A.accs[j].word && aw < A.accs[j].word + nw) v = acc_identity(A.accs[j].op, aw - A.accs[j].word);
-      }
-    }
-    reinterpret_cast<uint64_t*>(A.table)[i] = v;
-  }
-}
-// direct-key tables: the list of occupied entries (any order), counted into *counter
-__global__ void agg_build_occ_kernel(AggParams A, unsigned long long* counter) {
-  const uint64_t n_entries = A.capacity_mask + 2;
-  const uint64_t rounded = (n_entries + 31) & ~(uint64_t)31;
-  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < rounded; i += (uint64_t)gridDim.x * blockDim.x) {
-    bool occ = false;
-    if (i < n_entries) {
-      const uint64_t* e = reinterpret_cast<const uint64_t*>(A.table) + i * A.entry_words;
-      occ = i <= A.capacity_mask ? e[2] != DIRECT_EMPTY_KEY : e[0] != 0ull;
-    }
-    const unsigned m = __ballot_sync(0xFFFFFFFFu, occ);
-    if (m) {
-      const unsigned lane = threadIdx.x & 31;
-      unsigned long long base = 0;
-      if (lane == 0) base = atomicAdd(counter, (unsigned long long)__popc(m));
-      base = __shfl_sync(0xFFFFFFFFu, base, 0);
-      if (occ) A.occ[base + __popc(m & ((1u << lane) - 1))] = (uint32_t)i;
-    }
-  }
-}
-
 // grow: move every READY entry of `old` into the (larger, empty) table of `A`
 __global__ void agg_rehash_kernel(AggParams A, const uint8_t* old_table, const uint32_t* old_occ, uint64_t old_groups, uint32_t* err) {
   for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < old_groups; i += (uint64_t)gridDim.x * blockDim.x) {
@@ -2219,17 +2153,6 @@ cudaError_t launch_agg_migrate(const AggParams& A_new, const AggMigrateMap& M, c
   if (old_groups == 0) return cudaSuccess;
   int grid = (int)std::min<uint64_t>((old_groups + 255) / 256, grid_cap(8));
   agg_migrate_kernel<<<grid, 256, 0, s>>>(A_new, M, old_table, old_occ, old_groups, err);
-  return cudaGetLastError();
-}
-cudaError_t launch_agg_init_direct(const AggParams& A, cudaStream_t s) {
-  const uint64_t n_entries = A.capacity_mask + 2;
-  const uint64_t words = n_entries * A.entry_words;
-  agg_init_direct_kernel<<<(int)std::min<uint64_t>((words + 255) / 256, grid_cap(16)), 256, 0, s>>>(A, n_entries);
-  return cudaGetLastError();
-}
-cudaError_t launch_agg_build_occ(const AggParams& A, unsigned long long* counter, cudaStream_t s) {
-  const uint64_t n_entries = A.capacity_mask + 2;
-  agg_build_occ_kernel<<<(int)std::min<uint64_t>((n_entries + 255) / 256, grid_cap(16)), 256, 0, s>>>(A, counter);
   return cudaGetLastError();
 }
 cudaError_t launch_agg_extract(const AggParams& A, const AggExtractParams& X, uint64_t n_groups, uint32_t* err, cudaStream_t s) {

@@ -569,16 +569,4 @@ cudaError_t launch_rebase_views(void* views, int64_t n, uint64_t heap_base, cuda
   return cudaGetLastError();
 }
 
-__global__ void multi_copy_kernel(const CopySeg* __restrict__ segs, int n) {
-  for (int s = blockIdx.x; s < n; s += gridDim.x) {
-    const CopySeg g = segs[s];
-    for (unsigned long long i = threadIdx.x; i < g.bytes; i += blockDim.x) g.dst[i] = g.src[i];
-  }
-}
-cudaError_t launch_multi_copy_raw(const CopySeg* dev_segs, int n, cudaStream_t s) {
-  if (n == 0) return cudaSuccess;
-  multi_copy_kernel<<<std::min(n, grid_cap(4)), 256, 0, s>>>(dev_segs, n);
-  return cudaGetLastError();
-}
-
 }  // namespace sg

@@ -78,9 +78,6 @@ cudaError_t launch_assign_groups(const uint32_t* idx, const uint32_t* heads, con
 cudaError_t launch_iota(int64_t* out, int64_t n, cudaStream_t s);
 cudaError_t launch_iota_stride(int64_t* out, int64_t first, int64_t stride, int64_t n, cudaStream_t s);
 cudaError_t launch_widen_u32(const uint32_t* in, int64_t* out, int64_t n, cudaStream_t s);
-// many small device-to-device copies in one launch (packed exchange messages)
-struct CopySeg { const uint8_t* src; uint8_t* dst; unsigned long long bytes; };
-cudaError_t launch_multi_copy_raw(const CopySeg* dev_segs, int n, cudaStream_t s);
 cudaError_t launch_rebase_views(void* views, int64_t n, uint64_t heap_base, cudaStream_t s);
 
 }  // namespace sg

@@ -151,7 +151,7 @@ struct PipelineRunner {
     P.mask_slot = cp.mask_slot;
     P.error_flag = scal.error();
     P.n_probes = cp.n_probes;
-    bool tma = getenv("SAILGPU_NO_TMA") == nullptr;
+    bool tma = true;
     SG_CHECK(row0 % 1024 == 0, SAILGPU_ERR_INVALID, "chunk offset must be a multiple of 1024 rows");
     for (size_t i = 0; i < cp.inputs.size(); ++i) {
       const InputReg& r = cp.inputs[i];

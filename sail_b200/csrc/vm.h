@@ -113,8 +113,6 @@ struct AccDesc {
   uint32_t value_slot;     // NO_SLOT for count(*)
   uint32_t valid_slot;     // NO_SLOT => never null
   uint16_t word;           // first 8-byte word of this accumulator inside a global table entry
-  uint16_t pword;          // first word inside the thread-private (shared memory) block: sums are kept
-                           // as 64-bit partials there and spilled to the table entry on overflow
 };
 
 // One 8-byte word of the packed group key: where it is loaded from (static indexing => registers).
@@ -139,7 +137,6 @@ struct KeyDesc {
 // Global group table: state[capacity] (u32: 0 empty / 1 being written / 2 ready) kept apart so that a
 // worst-case-sized table costs only a 4-byte memset per slot; entries (AoS, written when claimed):
 //   [u32 tag | u32 pad][u64 seen][key words][acc words]
-constexpr unsigned long long DIRECT_EMPTY_KEY = 0x8000000000000000ull;
 struct AggParams {
   int32_t n_keys, n_accs;
   int32_t key_words;       // 8-byte words of packed key (incl. leading null-mask word if has_null_word)
@@ -149,8 +146,6 @@ struct AggParams {
   KeyDesc keys[MAX_KEYS];
   KeyWord kwords[MAX_KEY_WORDS];
   AccDesc accs[MAX_ACCS];
-  int32_t priv_words;      // (unused by the kernels; kept for layout stability)
-  int32_t priv_seen;
   int32_t reg_path;        // all accumulators are integer sums/counts: per-thread REGISTER partials for the first
                            // REG_GROUPS hot groups (no shuffles, no shared-memory traffic per row)
   int32_t kw_simple;       // every packed key word is a plain 8-byte load of a never-null column
@@ -164,12 +159,6 @@ struct AggParams {
   uint32_t hot_smem_off;   // arena offset of the hot-path scratch
   unsigned long long* n_groups;   // number of occupied entries
   int32_t cold_only;       // high-cardinality variant: no CTA dictionary, every row goes straight to the global table
-  // Direct-key protocol (tables whose packed key is ONE 8-byte word: a single integer / date / narrow-decimal / float key that is
-  // never null).  Every entry is pre-initialised to [0, 0, DIRECT_EMPTY_KEY, accumulator identities]; a slot is claimed by ONE
-  // 64-bit compare-and-swap on its key word -- no state word, no lock, no release fence, no acquire loads (the fence and the
-  // counter round trip are most of a 15 M-group aggregation's stall samples).  The one key equal
-  // to the sentinel lives in an extra entry behind the table.  `occ` is built by a scan before extraction / re-hashing.
-  int32_t direct_key;
   // Bounded table: the table is sized for the groups the operator expects, not for its input rows.  A CTA that sees
   // *n_groups above group_limit stops taking tiles and appends the ones it still owned to `deferred`; the host grows the
   // table and re-launches over that list.  group_limit leaves room for every tile that can still be in flight.

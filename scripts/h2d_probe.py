@@ -91,15 +91,12 @@ def main():
         print(json.dumps({"numa_node_of_source_pages": str(e)}), flush=True)
     run("warm-up", {})
     run("default (one pass, 256 Ki-row pieces, packers on the source's NUMA node)", {})
-    run("two passes (scan, then pack)", {"SAILGPU_PACK_ONE_PASS": "0"})
     run("packers NOT bound to the source's NUMA node", {"SAILGPU_PACK_NUMA": "0"})
     run("raw bytes (no packing)", {"SAILGPU_H2D_PACK": "0"})
     for th in (8, 16, 32):
         run(f"threads={th}", {"SAILGPU_PACK_THREADS": str(th)})
     for pr in (32768, 131072, 262144):
         run(f"piece_rows={pr}", {"SAILGPU_PACK_PIECE_ROWS": str(pr)})
-    run("host side only (dry)", {"SAILGPU_PACK_DRY": "1"})
-    run("host side only (dry), threads=32", {"SAILGPU_PACK_DRY": "1", "SAILGPU_PACK_THREADS": "32"})
     for name, cpus in nodes.items():
         aff = set()
         for part in cpus.split(","):
@@ -108,7 +105,6 @@ def main():
         aff &= os.sched_getaffinity(0)
         if aff:
             run(f"pinned to {name}", {}, aff)
-            run(f"pinned to {name}, dry", {"SAILGPU_PACK_DRY": "1"}, aff)
     # plain copies for scale: pageable and pinned cudaMemcpy of one 960 MB column
     import numpy as np
     col = table.column(0).chunks[0].buffers()[1]

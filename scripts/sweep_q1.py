@@ -20,7 +20,7 @@ def main():
     n = table.num_rows
     configs = [dict(), dict(SAILGPU_RPT="1", SAILGPU_STAGES="2"), dict(SAILGPU_RPT="4", SAILGPU_STAGES="1")]
     for cfg in configs:
-        for k in ("SAILGPU_RPT", "SAILGPU_STAGES", "SAILGPU_HOT", "SAILGPU_NO_TMA", "SAILGPU_MINB"):
+        for k in ("SAILGPU_RPT", "SAILGPU_STAGES", "SAILGPU_HOT", "SAILGPU_MINB"):
             os.environ.pop(k, None)
         os.environ.update(cfg)
         try:

@@ -1,6 +1,6 @@
 """GPU parity of the SPECIALISED aggregate kernel across group-key shapes.  The key travels in registers as G::Key (jit.cu,
 jit_rt.cuh), padded to the dictionary's four words: Q1's two Utf8View keys (four words, register tier), a nullable key
-(a null-mask word in front), a single 8-byte key (direct-key table), a float sum (dictionary tier) and three Decimal128
+(a null-mask word in front), a single 8-byte key (one-word global table), a float sum (dictionary tier) and three Decimal128
 keys (six words: wider than the dictionary, global table only).  Specialisation is forced from the first row; batch sizes
 include a partial last tile and more tiles than CTAs."""
 import decimal

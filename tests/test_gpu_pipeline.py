@@ -246,14 +246,17 @@ def test_aggregate_many_groups_multi_batch_growth():
 
 @pytest.mark.parametrize("late_nulls", [False, True])
 @pytest.mark.parametrize("ktype", ["int64", "date32", "decimal"])
-@pytest.mark.parametrize("direct", ["1", "0"])
-def test_aggregate_single_word_key_direct_protocol(ktype, late_nulls, direct, monkeypatch):
-    """One never-null 8-byte key word: with SAILGPU_DIRECT_KEY=1 slots are claimed by a compare-and-swap on the key word itself
-    (vm.h direct_key; opt-in, see engine.cu for the measurement); without it the general protocol runs the same input.  Covers the
-    sentinel value as a real key (INT64_MIN), growth with re-hashing over many batches, min/max identities, and a late batch with
-    NULL keys, which moves the table to the general layout (null-mask word) in the middle of the stream."""
+@pytest.mark.parametrize("kernel", ["interpreted", "specialised"])
+def test_aggregate_single_word_key(ktype, late_nulls, kernel, monkeypatch):
+    """One never-null 8-byte key word, in the interpreted and in the specialised kernel (whose global table is compiled for a
+    one-word key).  Covers INT64_MIN and 0 as real keys, growth with re-hashing over many batches, min/max identities, and a
+    late batch with NULL keys, which moves the table to a layout with a null-mask word in the middle of the stream."""
     from sail_b200 import engine
-    monkeypatch.setenv("SAILGPU_DIRECT_KEY", direct)
+    if kernel == "interpreted":
+        monkeypatch.setenv("SAILGPU_JIT", "0")
+    else:
+        monkeypatch.setenv("SAILGPU_JIT_MIN_ROWS", "0")
+        monkeypatch.setenv("SAILGPU_JIT_STRICT", "1")
     rng = np.random.default_rng(11)
     n_batches, n = 12, 50000
     batches = []
@@ -284,8 +287,10 @@ def test_aggregate_single_word_key_direct_protocol(ktype, late_nulls, direct, mo
         op.push(t)
     op.finish()
     got = op.collect()
+    m = op.metrics()
     op.close()
     assert_same(got, oracle_op(spec, whole))
+    assert (m.get("gpu.jit_launches", 0) > 0) == (kernel == "specialised"), m
 
 
 @pytest.mark.parametrize("nulls", [False, True])

@@ -294,16 +294,14 @@ def test_hot_path_every_aggregate(nulls, no_regpath, kernel, monkeypatch):
     run_agg_case(t, cols, AVG_AGGS, kernel)
 
 
-@pytest.mark.parametrize("mode", ["many_groups", "first_limit_0", "direct_key"])
+@pytest.mark.parametrize("mode", ["many_groups", "first_limit_0", "extreme_keys"])
 def test_cold_path_every_aggregate(mode, kernel, monkeypatch):
     """the global table: many groups over several batches (the table grows while streaming), a forced hand-back after the first
-    pass, and the direct-key protocol with INT64_MIN among the keys"""
+    pass, and a never-null Int64 key with INT64_MIN, INT64_MAX and -1 among the keys"""
     if mode == "first_limit_0":
         monkeypatch.setenv("SAILGPU_AGG_FIRST_LIMIT", "0")
-    if mode == "direct_key":
-        monkeypatch.setenv("SAILGPU_DIRECT_KEY", "1")
-    t, cols = agg_case(60_007, 20_000, mode != "direct_key", 14)
-    if mode == "direct_key":
+    t, cols = agg_case(60_007, 20_000, mode != "extreme_keys", 14)
+    if mode == "extreme_keys":
         k = cols["k"][0]
         k[:3] = [W.I64_MIN, W.I64_MAX, -1]
         t = t.set_column(0, "k", W.array(k, "Int64"))
