@@ -37,7 +37,10 @@
  *   {"op":"projection","exprs":[{"expr":E,"name":"..."},...]}
  *   {"op":"aggregate","mode":"partial|final|final_partitioned|single",
  *    "group_by":[{"expr":E,"name":".."}],"aggs":[{"fn":"sum|avg|count|min|max","args":[E],
- *    "name":"..","input_type":"T"}]}
+ *    "name":"..","input_type":"T","distinct":false|true}]}
+ *                                          ("distinct": true -- count / sum / avg(DISTINCT E) -- in mode single only, over one
+ *                                           argument that is not Float32 / Float64 / Boolean, at most 4 distinct arguments per
+ *                                           aggregate; for min / max the flag is a no-op)
  *   {"op":"hash_join","join_type":"inner|left|right|left_semi|left_anti|right_semi|right_anti","on":[[l,r],...],
  *    "filter":E|null,"projection":[...]|null}   (input 0 = build = LEFT child, input 1 = probe; residual filters with
  *                                           inner, right_semi, left_semi and left_anti)

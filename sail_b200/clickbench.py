@@ -14,6 +14,8 @@ nothing falls back):
   21, 22  MIN(URL) / MIN(Title): min/max over strings (planned below as REJECTED, the tests pin the plan-time error)
   27      length(URL): character_length, planned in LENGTH_QUERIES
   28      regexp_replace(): a scalar string function outside {substr, like, character_length}
+[09] runs in QUERIES as the two-level rewrite c9; DISTINCT_QUERIES['c9_single'] is the reference's own shape, one single-mode
+aggregate with count(DISTINCT UserID) next to the plain aggregates.
 Strings are Utf8View and EventTime is Int64 seconds (see datagen/hits.py); [23] `SELECT *` selects ten columns, [29] runs as six aggregates.
 """
 from __future__ import annotations
@@ -111,6 +113,17 @@ def c9():
                                             ("count", col("alias1"), "count(DISTINCT UserID)", I64)])
     avg = binop("/", {"cast": col("rs"), "to": "Float64"}, {"cast": col("rn"), "to": "Float64"})
     p = project(outer, ["RegionID", "sum(AdvEngineID)", "c", (avg, "avg(ResolutionWidth)"), "count(DISTINCT UserID)"])
+    return sort(p, [("c", False)], fetch=10)
+
+
+def c9_single():
+    """[09] in the reference's plan shape (test_clickbench.plan.yaml [09]): one single-mode aggregate by RegionID with
+    count(DISTINCT UserID) next to the plain aggregates -- the DISTINCT accumulator runs behind a per-(RegionID, UserID) gate on
+    the GPU -- then the projection and TopK(fetch=10) on c"""
+    a = aggregate(hits(["RegionID", "UserID", "AdvEngineID", "ResolutionWidth"]), "single", ["RegionID"],
+                  [("sum", col("AdvEngineID"), "sum(AdvEngineID)", I16), ("count", None, "c", None), ("avg", col("ResolutionWidth"), "avg(ResolutionWidth)", I16),
+                   ("count", col("UserID"), "count(DISTINCT UserID)", I64, True)])
+    p = project(a, ["RegionID", "sum(AdvEngineID)", "c", "avg(ResolutionWidth)", "count(DISTINCT UserID)"])
     return sort(p, [("c", False)], fetch=10)
 
 
@@ -370,5 +383,7 @@ REJECTED = {"c21": Query(c21, 21, order=("c",)), "c22": Query(c22, 22, order=("c
 TIMESTAMP_QUERIES = {"c18": Query(c18, 18, order=("count(*)",)), "c42": Query(c42, 42, order=("M",), skip=1000)}
 # [27] needs character_length: planned outside QUERIES as well
 LENGTH_QUERIES = {"c27": Query(c27, 27, order=("l",), floats=(1,), params=("min_count",))}
+# [09] as the reference plans it (a DISTINCT aggregate next to plain ones, mode single); QUERIES keeps the two-level rewrite c9
+DISTINCT_QUERIES = {"c9_single": Query(c9_single, 9, order=("c",), floats=(3,))}
 NOT_PLANNED = {18: "extract(minute FROM Timestamp): TIMESTAMP_QUERIES['c18']", 27: "length(URL): LENGTH_QUERIES['c27']", 28: "regexp_replace(Referer, ..)",
                42: "date_trunc('minute', Timestamp): TIMESTAMP_QUERIES['c42']"}

@@ -376,6 +376,35 @@ void PipelineCompiler::finish_aggregate(CompiledPipeline& out, const StageSpec& 
     return A.n_accs++;
   };
   auto ident = [&](const std::string& what, int j) { out.acc_ident[what] = j; return j; };
+  // DISTINCT: one gate per argument (shared by count / sum / avg over it), a B slot that is true on the one row of each
+  // (group key, argument) pair that claimed the pair in the argument's pair set.  The gate implies an active row and a valid
+  // argument, so it alone is the validity of the gated accumulators: that slot is new, so add_acc never merges a gated
+  // accumulator with a plain one over the same argument, and their identities carry "distinct|".
+  std::map<std::string, int> gates;
+  auto gate_for = [&](const Val& x0, const DataType& t, const std::string& id) -> int {
+    auto it = gates.find(id);
+    if (it != gates.end()) return it->second;
+    SG_CHECK((int)out.distinct.size() < MAX_DISTINCT, SAILGPU_ERR_UNSUPPORTED, "more than " + std::to_string(MAX_DISTINCT) + " DISTINCT arguments in one aggregate");
+    const Val x = ensure_slot(x0);
+    AggParams D{};
+    D.n_keys = A.n_keys + 1;
+    SG_CHECK(D.n_keys <= MAX_KEYS, SAILGPU_ERR_UNSUPPORTED, "DISTINCT aggregate: grouping columns plus the argument exceed " + std::to_string(MAX_KEYS) + " columns");
+    for (int i = 0; i < A.n_keys; ++i) D.keys[i] = A.keys[i];
+    D.keys[A.n_keys] = key_desc(x, t);
+    D.has_null_word = 1;            // always: the pair layout does not depend on which batches carry validity buffers
+    D.key_words = 1;
+    for (int i = 0; i < D.n_keys; ++i) D.key_words += D.keys[i].width == 16 ? 2 : 1;
+    SG_CHECK(D.key_words <= MAX_KEY_WORDS, SAILGPU_ERR_UNSUPPORTED, "DISTINCT aggregate: grouping columns plus the argument are wider than " + std::to_string(MAX_KEY_WORDS * 8 - 8) + " bytes");
+    D.entry_words = (uint32_t)(2 + D.key_words);
+    D.group_limit = ~0ull;
+    Val g = temp(K_B);
+    VmInst I{}; I.op = OP_DISTINCT_FIRST; I.aux = (uint16_t)out.distinct.size(); I.dst = (uint32_t)g.slot; I.a = I.b = NO_SLOT;
+    I.c = (!mask_.is_imm && mask_.slot >= 0) ? (uint32_t)mask_.slot : NO_SLOT;
+    prog_.push_back(I);
+    out.distinct.push_back(D);
+    gates[id] = g.slot;
+    return g.slot;
+  };
   auto sum_acc = [&](const Val& x, const DataType& t, const std::string& id) -> int {
     if (t.is_decimal()) { const int j = add_acc(ACC_SUM_I128, &x); if (t.precision <= 16 && j < MAX_ACCS) small_acc_[j] = true; return ident("sum|" + id, j); }
     if (t.is_float()) { Val f = convert(x, K_F64); f.vslot = x.vslot; return ident("sum|" + id, add_acc(ACC_SUM_F64, &f)); }
@@ -411,7 +440,20 @@ void PipelineCompiler::finish_aggregate(CompiledPipeline& out, const StageSpec& 
       AggOutSpec o{}; o.kind = kind; o.a = x; o.b = y; o.type = t; o.nullable = nullable; o.in_type = in_t;
       out.agg_outs.push_back(o);
     };
-    if (a.fn == "count") {
+    Val xg;             // DISTINCT: the argument behind its gate
+    if (a.distinct) { xg = ensure_slot(arg); xg.vslot = gate_for(arg, in_t, aid); }
+    if (a.distinct && a.fn == "count") {
+      push_out(1, ident("count|distinct|" + aid, add_acc(ACC_COUNT, &xg)), 0, T(TypeId::Int64), false);
+    } else if (a.distinct && a.fn == "sum") {
+      const int j = sum_acc(xg, in_t, "distinct|" + aid);
+      push_out(1, j, 0, at.state[0], A.accs[j].track_seen != 0);
+    } else if (a.distinct && a.fn == "avg") {
+      const int jc = ident("count|distinct|" + aid, add_acc(ACC_COUNT, &xg));
+      int js;
+      if (in_t.is_decimal()) js = sum_acc(xg, in_t, "distinct|" + aid);
+      else { Val f = convert(xg, K_F64); f.vslot = xg.vslot; js = ident("sumf|distinct|" + aid, add_acc(ACC_SUM_F64, &f)); }
+      push_out(2, js, jc, at.final_type, true);
+    } else if (a.fn == "count") {
       int j;
       if (merging) { Val s = state_val(0); Val w = convert(s, K_I64); w.vslot = s.vslot; j = add_acc(ACC_SUM_I64, &w); A.accs[j].track_seen = 0; }
       else if (has_arg && arg.vslot >= 0) { Val only_valid = arg; j = add_acc(ACC_COUNT, &only_valid); }
@@ -590,6 +632,8 @@ void PipelineCompiler::finalize(CompiledPipeline& out, Ctx* ctx, int hot_wanted)
     for (int i = 0; i < AA.n_keys; ++i) { AA.keys[i].slot = off(AA.keys[i].slot); AA.keys[i].valid_slot = off(AA.keys[i].valid_slot); }
     for (int w = AA.has_null_word; w < AA.key_words; ++w) { AA.kwords[w].slot = off(AA.kwords[w].slot); AA.kwords[w].valid_slot = off(AA.kwords[w].valid_slot); }
     for (int j = 0; j < AA.n_accs; ++j) { AA.accs[j].value_slot = off(AA.accs[j].value_slot); AA.accs[j].valid_slot = off(AA.accs[j].valid_slot); }
+    for (AggParams& D : out.distinct)
+      for (int i = 0; i < D.n_keys; ++i) { D.keys[i].slot = off(D.keys[i].slot); D.keys[i].valid_slot = off(D.keys[i].valid_slot); }
     for (int j = 0; j < AA.n_accs && j < REG_ACCS; ++j) {
       AA.rload[j].slot = AA.accs[j].value_slot; AA.rload[j].stride = AA.accs[j].stride;
       AA.rload[j].mode = (uint8_t)(AA.accs[j].op == ACC_COUNT ? 0 : AA.accs[j].vkind == K_I64 ? (small_acc_[j] ? 3 : 1) : 2);

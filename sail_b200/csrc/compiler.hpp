@@ -38,7 +38,8 @@ struct StageSpec {
   // Aggregate
   std::string mode;
   std::vector<ExprPtr> group_exprs; std::vector<std::string> group_names;
-  struct Agg { std::string fn, name; ExprPtr arg; DataType input_type; bool has_arg = false; };
+  // distinct: count / sum / avg(DISTINCT arg) of a single-mode aggregate (the flag of min / max is dropped while parsing)
+  struct Agg { std::string fn, name; ExprPtr arg; DataType input_type; bool has_arg = false; bool distinct = false; };
   std::vector<Agg> aggs;
 };
 
@@ -75,6 +76,7 @@ struct CompiledPipeline {
   std::vector<DataType> out_types;
   AggParams agg{};                   // SINK_AGG (table pointers filled at launch)
   std::vector<AggOutSpec> agg_outs;
+  std::vector<AggParams> distinct;   // SINK_AGG: the pair set of every DISTINCT argument (OP_DISTINCT_FIRST aux = index; tables filled at launch)
   std::map<std::string, int> acc_ident;   // SINK_AGG: "what is accumulated" (function | argument expression) -> accumulator index; the same
                                      // identities exist under every validity signature, which is how a table is carried over when a
                                      // later batch brings validity buffers an earlier one did not have (engine.cu: migrate_layout)

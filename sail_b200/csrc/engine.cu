@@ -20,6 +20,30 @@ __global__ void agg_counters_kernel(const unsigned long long* __restrict__ scal,
 // ------------------------------------------------------------------------------------------------
 // spec parsing
 // ------------------------------------------------------------------------------------------------
+// An aggregate's "distinct": true (DataFusion's AggregateFunctionExpr::is_distinct).  count / sum / avg over one argument of a
+// single-mode aggregate run as accumulators behind a per-pair gate (compiler.cu finish_aggregate); for min / max the flag
+// changes nothing and is dropped, as in DataFusion.  Everything else is refused here, while planning.
+static int pair_key_words(const DataType& t) { return t.is_string() || (t.is_decimal() && t.precision > 18) ? 2 : 1; }
+static void check_distinct(const StageSpec& st, StageSpec::Agg& ag, const Json* args, std::set<std::string>* distinct_args) {
+  const std::string what = ag.fn + "(DISTINCT) '" + ag.name + "'";
+  SG_CHECK(st.mode == "single", SAILGPU_ERR_UNSUPPORTED, what + " in mode '" + st.mode + "' is not supported on the GPU path: DataFusion's partial state of a DISTINCT aggregate is a List column");
+  const size_t n_args = args && args->kind == Json::Arr ? args->a.size() : 0;
+  SG_CHECK(n_args > 0, SAILGPU_ERR_INVALID, what + " needs an argument");
+  SG_CHECK(n_args == 1, SAILGPU_ERR_UNSUPPORTED, what + " over more than one argument is not supported on the GPU path");
+  if (ag.fn == "min" || ag.fn == "max") return;
+  SG_CHECK(ag.fn == "count" || ag.fn == "sum" || ag.fn == "avg", SAILGPU_ERR_UNSUPPORTED, "aggregate function '" + ag.fn + "' with DISTINCT");
+  const DataType& t = ag.arg->type;
+  SG_CHECK(!t.is_float() && t.id != TypeId::Bool, SAILGPU_ERR_UNSUPPORTED, what + " over " + t.str() + " is not supported on the GPU path");
+  // the pair set's key: a null-mask word, the group keys, the argument (compiler.cu gate_for)
+  int words = 1 + pair_key_words(t);
+  for (auto& g : st.group_exprs) words += pair_key_words(g->type);
+  SG_CHECK((int)st.group_exprs.size() + 1 <= MAX_KEYS && words <= MAX_KEY_WORDS, SAILGPU_ERR_UNSUPPORTED,
+           what + ": the grouping columns and the argument take more than " + std::to_string(MAX_KEYS) + " columns or " + std::to_string(MAX_KEY_WORDS * 8) + " bytes of pair key");
+  distinct_args->insert(ag.arg->key());
+  SG_CHECK((int)distinct_args->size() <= MAX_DISTINCT, SAILGPU_ERR_UNSUPPORTED, "more than " + std::to_string(MAX_DISTINCT) + " DISTINCT arguments in one aggregate");
+  ag.distinct = true;
+}
+
 StageSpec parse_stage(const Json& j, const Schema& in, Schema* out) {
   StageSpec st;
   const std::string op = j.at("op").as_str();
@@ -59,6 +83,7 @@ StageSpec parse_stage(const Json& j, const Schema& in, Schema* out) {
       out->push_back({st.group_names.back(), e->type, e->nullable});
     }
     size_t state_col = st.group_exprs.size();
+    std::set<std::string> distinct_args;
     for (auto& a : j.at("aggs").a) {
       StageSpec::Agg ag;
       ag.fn = a.at("fn").as_str();
@@ -68,6 +93,11 @@ StageSpec parse_stage(const Json& j, const Schema& in, Schema* out) {
       const Json* args = a.find("args");
       if (!merging && args && args->kind == Json::Arr && !args->a.empty()) { ag.arg = parse_expr(args->a[0], in); ag.has_arg = true; ag.input_type = ag.arg->type; }
       SG_CHECK(ag.fn == "count" || ag.has_arg || merging, SAILGPU_ERR_INVALID, "aggregate '" + ag.fn + "' needs an argument");
+      const Json* ds = a.find("distinct");
+      if (ds && !ds->is_null()) {
+        SG_CHECK(ds->kind == Json::Bool, SAILGPU_ERR_INVALID, "aggregate '" + ag.name + "': \"distinct\" must be true or false");
+        if (ds->b) check_distinct(st, ag, args, &distinct_args);
+      }
       SG_CHECK(ag.fn == "count" || ag.input_type.id != TypeId::Null, SAILGPU_ERR_INVALID, "aggregate '" + ag.name + "' needs input_type in final mode");
       AggTypes at = agg_types(ag.fn, ag.fn == "count" ? T(TypeId::Int64) : ag.input_type);
       if (merging) {
@@ -354,6 +384,40 @@ struct PipelineOp : Op {
     }
   }
 
+  // ---- DISTINCT aggregates: pair sets ---------------------------------------------------------------
+  // One set per DISTINCT argument (compiler.cu gate_for), a group table without accumulators.  A set is never emptied (not
+  // by a spill either), grows like the group table -- bounded, with hand-backs -- and is not partitioned: past max_capacity()
+  // the aggregate is refused.
+  std::vector<AggTable> dsets;
+  BufPtr dcounts;                      // the pair count of every set
+  unsigned long long* pair_count(size_t d) { return static_cast<unsigned long long*>(dcounts->ptr) + d; }
+
+  void alloc_set(size_t d, const AggParams& D0, uint64_t cap, uint64_t pairs) {
+    SG_CHECK(cap <= max_capacity(), SAILGPU_ERR_UNSUPPORTED, "count(DISTINCT) needs more than " + std::to_string(max_capacity()) + " pair slots");
+    AggTable old = dsets[d];
+    AggTable& t = dsets[d];
+    t.capacity = cap;
+    t.table = dev_alloc(ctx, (size_t)cap * D0.entry_words * 8);
+    t.state = dev_alloc_zero(ctx, (size_t)cap * 4);
+    t.occ = dev_alloc(ctx, (size_t)cap * 4);
+    if (old.capacity && pairs) {
+      AggParams D = D0;
+      fill_set(D, d);
+      SG_CUDA(cudaMemsetAsync(pair_count(d), 0, 8, ctx->stream));
+      SG_CUDA(launch_agg_rehash(D, static_cast<const uint8_t*>(old.table->ptr), static_cast<const uint32_t*>(old.occ->ptr), pairs, run.scal.error(), ctx->stream));
+      m.kernel_launches++;
+    }
+  }
+  void fill_set(AggParams& D, size_t d) {
+    const AggTable& t = dsets[d];
+    D.table = static_cast<uint8_t*>(t.table->ptr);
+    D.state = static_cast<uint32_t*>(t.state->ptr);
+    D.occ = static_cast<uint32_t*>(t.occ->ptr);
+    D.capacity_mask = t.capacity - 1;
+    D.n_groups = pair_count(d);
+    D.group_limit = ~0ull;           // launch() derives it from the grid
+  }
+
   // one launch over all tiles of `b` (list == null) or over the listed tiles; tiles handed back land in `deferred_out`
   void launch_agg(const std::shared_ptr<CompiledPipeline>& cp, const DevBatch& b, const BufPtr& list, int64_t n_list, const BufPtr& deferred_out, int slot) {
     PipelineParams P;
@@ -363,6 +427,10 @@ struct PipelineOp : Op {
     memset(&aux, 0, sizeof(aux));
     aux.agg = cp->agg;
     fill_table(aux.agg);
+    std::vector<AggParams> sets = cp->distinct;       // host copy: launch() rebases it per stage and uploads it
+    for (size_t d = 0; d < sets.size(); ++d) fill_set(sets[d], d);
+    aux.distinct = sets.data();
+    aux.n_distinct = (int32_t)sets.size();
     if (deferred_out) {
       if (!(next_zeroed && !list)) SG_CUDA(cudaMemsetAsync(n_deferred_ptr(slot), 0, 8, ctx->stream));
       next_zeroed = false;
@@ -463,17 +531,26 @@ struct PipelineOp : Op {
     }
     agg_cp = cp;
     const bool grouped = cp->agg.n_keys > 0;
+    // a pair set is bounded like a group table, so an aggregate with DISTINCT hands tiles back even without group keys
+    const bool guarded = grouped || !cp->distinct.empty();
+    if (dsets.empty() && !cp->distinct.empty()) {
+      dsets.resize(cp->distinct.size());
+      dcounts = dev_alloc_zero(ctx, MAX_DISTINCT * 8);
+      const uint64_t cap = std::min<uint64_t>(std::min<uint64_t>(min_capacity(), max_capacity()), next_pow2(8 * (uint64_t)b->rows + 2048));
+      for (size_t d = 0; d < dsets.size(); ++d) alloc_set(d, cp->distinct[d], cap, 0);
+    }
     // first table: 4 M slots for real inputs, but a final aggregate over a few partial rows gets a few KB (a hand-back
     // grows it if later batches are bigger)
     if (!tab.capacity) alloc_table(cp->agg, grouped ? std::min<uint64_t>(std::min<uint64_t>(min_capacity(), max_capacity()), next_pow2(8 * (uint64_t)b->rows + 2048)) : 1024, 0);
     const int64_t tile_rows = (int64_t)cp->rpt * NT;
     const int64_t n_tiles = (b->rows + tile_rows - 1) / tile_rows;
-    BufPtr deferred = grouped ? dev_alloc(ctx, (size_t)n_tiles * 4) : nullptr;
+    BufPtr deferred = guarded ? dev_alloc(ctx, (size_t)n_tiles * 4) : nullptr;
     const int slot = next_slot;
     launch_agg(cp, *b, nullptr, 0, deferred, slot);
     rows_in_table += b->rows;
+    rows_seen_by_sets += b->rows;
     known_groups = -1;
-    if (!grouped) return;
+    if (!guarded) return;
     next_slot ^= 1;
     copy_counters(slot, true);
     inflight.push_back({b, cp, deferred, slot});
@@ -495,6 +572,31 @@ struct PipelineOp : Op {
     }
   }
 
+  int64_t rows_seen_by_sets = 0;      // rows pushed so far (rows_in_table restarts at a spill; the pair sets do not)
+
+  // grows every pair set that is past its limit or, by the pairs per row seen so far, would be after the deferred rows
+  void grow_sets(double rows_def) {
+    if (dsets.empty()) return;
+    std::vector<unsigned long long> pairs(dsets.size());
+    SG_CUDA(cudaMemcpyAsync(pairs.data(), dcounts->ptr, pairs.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    stream_sync(ctx);
+    const double rows_done = std::max(1.0, (double)rows_seen_by_sets - rows_def);
+    const uint64_t ceiling = max_capacity();
+    for (size_t d = 0; d < dsets.size(); ++d) {
+      const uint64_t p = pairs[d];
+      const double ratio = p ? std::min(1.0, (double)p / rows_done) : 1.0;
+      uint64_t cap = next_pow2((uint64_t)(2.0 * ((double)p + ratio * rows_def * 1.25 + 1024.0)));
+      const bool over = p > run.last_pair_limit[d];
+      if (over && cap <= dsets[d].capacity) cap = dsets[d].capacity * 2;
+      // the set is not partitioned: at the ceiling a set past its limit is refused before anything is allocated
+      if (cap > ceiling) {
+        SG_CHECK(!(over && dsets[d].capacity >= ceiling), SAILGPU_ERR_UNSUPPORTED, "count(DISTINCT) needs more than " + std::to_string(ceiling) + " pair slots");
+        cap = ceiling;
+      }
+      if (cap > dsets[d].capacity) alloc_set(d, agg_cp->distinct[d], cap, p);
+    }
+  }
+
   // Slow path: some launch in flight handed tiles back or raised an error.  Drains the stream, then, until nothing is left,
   // grows the table for every deferred tile at once and re-launches over each list.
   void resolve_all() {
@@ -502,6 +604,7 @@ struct PipelineOp : Op {
     stream_sync(ctx);
     const Counters* latest = &counters[inflight.back().slot];    // copied after the newest launch: the current values
     uint64_t prev_def = 0;
+    const bool grouped = agg_cp->agg.n_keys > 0;
     for (;;) {
       raise_device_error(ctx, run.scal.error(), latest->error);
       const uint64_t groups = latest->n_groups;
@@ -521,12 +624,14 @@ struct PipelineOp : Op {
       // a hand-back does not always mean a full table: the dictionary variant gives up at HOT_GROUP_LIMIT groups whatever the
       // capacity.  The table only grows when the estimate asks for it, or when a re-launch at this capacity made no progress.
       const bool stuck = prev_def != 0 && n_def_total >= prev_def;
-      if (cap <= tab.capacity && stuck) cap = tab.capacity * 2;
+      // (with pair sets a hand-back may have been for a set alone: then the group table does not double)
+      if (cap <= tab.capacity && stuck && (dsets.empty() || groups > run.last_group_limit)) cap = tab.capacity * 2;
       prev_def = n_def_total;
+      grow_sets(rows_def);
       // partitioned mode: the table grows to the ceiling and no further.  A full table at the ceiling hands its groups on as
       // state rows (spill) and starts over empty; the re-launches below then fill it again.
       const uint64_t ceiling = max_capacity();
-      if (cap > ceiling) {
+      if (cap > ceiling && grouped) {
         cap = ceiling;
         if (tab.capacity >= ceiling && groups) {
           SG_CHECK(!partition_of_parent, SAILGPU_ERR_UNSUPPORTED, "a partition of a partitioned aggregate needs more than 2^28 group slots");
@@ -535,7 +640,7 @@ struct PipelineOp : Op {
           prev_def = 0;
         }
       }
-      if (cap > tab.capacity) alloc_table(inflight.front().cp->agg, cap, groups);
+      if (cap > tab.capacity && grouped) alloc_table(inflight.front().cp->agg, cap, groups);
       if (!use_cold && groups > CARD_MANY_GROUPS) {
         auto cold = run.compiled_for(*inflight.front().batch, true);
         if (cold->agg.entry_words == inflight.front().cp->agg.entry_words) use_cold = true;     // later batches start on the many-groups variant
@@ -735,7 +840,9 @@ struct PipelineOp : Op {
         for (;;) { BatchPtr b; const bool more = rp->pull_partition((int)p, &b); if (b && b->rows) parts[(size_t)p].push_back(b); if (!more) break; }
       m.kernel_launches += rp->m.kernel_launches;
     }
-    // one final aggregate per partition over the state rows: [keys | states] -> the operator's output
+    // one final aggregate per partition over the state rows: [keys | states] -> the operator's output.  A DISTINCT aggregate
+    // merges as its plain counterpart (no "distinct" here): the pair sets were never emptied, so each pair was counted in
+    // exactly one state row, and a sum of counts / sums over the state rows is the DISTINCT result.
     Json gb; gb.kind = Json::Arr;
     for (int i = 0; i < n_keys; ++i) { Json g; g.kind = Json::Obj; g.o = {{"expr", jcol(i)}, {"name", jstr(st.group_names[(size_t)i])}}; gb.a.push_back(g); }
     Json aggs; aggs.kind = Json::Arr;

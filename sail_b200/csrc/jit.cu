@@ -414,6 +414,8 @@ bool jit_supported(const CompiledPipeline& cp, std::string* why) {
   // the interpreter issues the first-slot loads of all rows of a thread before the dependent key loads, and latency, not
   // instructions, bounds a probe
   if (cp.n_probes > 0) return no("join probes run on the interpreter");
+  // the gate of a DISTINCT aggregate (a pair-set lookup per row) is not generated yet
+  if (!cp.distinct.empty()) return no("DISTINCT aggregates (OP_DISTINCT_FIRST gates) run on the interpreter");
   return true;
 }
 

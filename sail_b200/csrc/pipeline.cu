@@ -513,6 +513,9 @@ __device__ __noinline__ void vm_gather(const VmInst& I, const TileCtx& c) {
 }
 
 template <int RPT>
+__device__ __noinline__ void vm_distinct_first(const AggParams& D, const TileCtx& c, uint32_t dst, uint32_t mask_slot, uint32_t* err);
+
+template <int RPT>
 __device__ __forceinline__ void vm_exec(const VmInst* prog, int n_inst, const TileCtx& c, const PipelineParams& P,
                                         const PipelineAux* aux) {
   for (int pc = 0; pc < n_inst; ++pc) {
@@ -697,6 +700,7 @@ __device__ __forceinline__ void vm_exec(const VmInst* prog, int n_inst, const Ti
       case OP_TS_TRUNC: vm_ts<RPT, true>(I, c); break;
       case OP_PROBE: vm_probe<RPT>(aux->probe[I.aux], c, I.c); break;
       case OP_GATHER: vm_gather<RPT>(I, c); break;
+      case OP_DISTINCT_FIRST: vm_distinct_first<RPT>(aux->distinct[I.aux], c, I.dst, I.c, P.error_flag); break;
       default: break;
     }
   }
@@ -736,7 +740,8 @@ __device__ __forceinline__ void load_tile_generic(const PipelineParams& P, uint8
 
 // state word: 0 = empty, else (tag30 << 2) | {1 = being written, 2 = ready}.  Carrying the tag in the
 // state lets a thread skip a slot that is being written for a different key without waiting on it.
-__device__ __forceinline__ uint64_t* agg_find_or_insert(const AggParams& A, const KeyRegs& key, uint64_t h, uint32_t* err) {
+// `claimed` (optional) is set when this call inserted the key: exactly one caller per key sees it.
+__device__ __forceinline__ uint64_t* agg_find_or_insert(const AggParams& A, const KeyRegs& key, uint64_t h, uint32_t* err, bool* claimed = nullptr) {
   const uint32_t tag = (uint32_t)(h >> 34) << 2;
   uint64_t idx = h & A.capacity_mask;
   uint64_t probes = 0;
@@ -755,6 +760,7 @@ __device__ __forceinline__ uint64_t* agg_find_or_insert(const AggParams& A, cons
           for (int w = 0; w < acc_words_of(A.accs[j].op); ++w)
             e[2 + A.key_words + A.accs[j].word + w] = acc_identity(A.accs[j].op, w);
         st_release_u32(st, tag | ST_READY);                         // release: the entry words above are visible first
+        if (claimed) *claimed = true;
         {
           // occupied-slot list: one counter for the whole table, so the increment is aggregated over the lanes
           // that insert in the same step (same-address atomics serialise in one L2 slice)
@@ -787,19 +793,42 @@ __device__ __forceinline__ uint64_t* agg_find_or_insert(const AggParams& A, cons
 // Warp-cooperative front end: lanes of one warp that carry the same key hash elect a leader
 // (__match_any_sync); only leaders touch the table, followers receive the entry pointer by shuffle.
 // Removes same-warp contention on a slot that is being published.  All 32 lanes must call.
-__device__ __forceinline__ uint64_t* agg_find_or_insert_warp(const AggParams& A, const KeyRegs& key, uint64_t h, bool need, uint32_t* err) {
+// `claimed` (optional): this lane's key was inserted by this call -- by the lane itself, never for a follower.
+__device__ __forceinline__ uint64_t* agg_find_or_insert_warp(const AggParams& A, const KeyRegs& key, uint64_t h, bool need, uint32_t* err, bool* claimed = nullptr) {
   const unsigned lane = threadIdx.x & 31;
   const unsigned long long probe = need ? h : (0xFFFFFFFF00000000ull | lane);   // idle lanes match nobody useful
   const unsigned peers = __match_any_sync(0xFFFFFFFFu, probe);
   const int leader = __ffs(peers) - 1;
   uint64_t* e = nullptr;
-  if (need && (int)lane == leader) e = agg_find_or_insert(A, key, h, err);
+  bool mine = false;
+  if (need && (int)lane == leader) e = agg_find_or_insert(A, key, h, err, &mine);
   unsigned long long p = __shfl_sync(0xFFFFFFFFu, reinterpret_cast<unsigned long long>(e), leader);
   uint64_t* got = reinterpret_cast<uint64_t*>(p);
   // same hash but different key (64-bit collision inside one warp): fall back to an own lookup
   if (need && (int)lane != leader && got && !key_words_equal(A.keys, A.n_keys, A.has_null_word, got + 2, key))
-    got = agg_find_or_insert(A, key, h, err);
+    got = agg_find_or_insert(A, key, h, err, &mine);
+  if (claimed) *claimed = mine;
   return need ? got : nullptr;
+}
+
+// OP_DISTINCT_FIRST: the gate of a DISTINCT aggregate.  Every active row with a valid argument looks its (group key, argument)
+// pair up in the pair set D (key: null-mask word, group keys, argument last); the row whose lookup inserted the pair passes.
+// The set is never emptied, so over the whole input exactly one row per pair passes, and the accumulators behind the gate
+// see every distinct argument of a group once.  Rows of one warp with the same pair share one lookup (the warp front end).
+template <int RPT>
+__device__ __noinline__ void vm_distinct_first(const AggParams& D, const TileCtx& c, uint32_t dst, uint32_t mask_slot, uint32_t* err) {
+  uint8_t* pd = c.arena + eff(c, dst);
+  const uint8_t* pact = mask_slot == NO_SLOT ? nullptr : c.arena + eff(c, mask_slot);
+  const uint32_t xv = D.keys[D.n_keys - 1].valid_slot;
+  for (int k = 0; k < RPT; ++k) {
+    const int r = threadIdx.x + k * NT;
+    const bool live = r < c.nrows && (pact == nullptr || pact[r]) && (xv == NO_SLOT || c.arena[eff(c, xv) + r]);
+    KeyRegs key; bool hn; uint64_t h = 0;
+    if (live) h = pack_key<MAX_KEYS>(D.keys, D.n_keys, 1, c, r, key, &hn);
+    bool first = false;
+    agg_find_or_insert_warp(D, key, h, live, err, &first);
+    pd[r] = first ? 1 : 0;
+  }
 }
 
 // hash of an already packed key (same value pack_key() returns for the row it was packed from)
@@ -1743,7 +1772,14 @@ __global__ void __launch_bounds__(NT, MINB) pipeline_kernel(const __grid_constan
   // bounded aggregation table (AggParams::group_limit): once the table is nearly full this CTA stops taking tiles
   const bool guarded = KC != KC_OTHER && K.aux[0].agg.deferred != nullptr;
   auto groups_now = [&]() -> unsigned long long { return *reinterpret_cast<volatile unsigned long long*>(K.aux[0].agg.n_groups); };
-  auto table_full = [&]() -> int { return groups_now() > K.aux[0].agg.group_limit ? 1 : 0; };
+  auto pairs_over = [&]() -> bool {                       // any pair set of a DISTINCT aggregate past its limit
+    for (int d = 0; d < K.aux[0].n_distinct; ++d) {
+      const AggParams& D = K.aux[0].distinct[d];
+      if (*reinterpret_cast<volatile unsigned long long*>(D.n_groups) > D.group_limit) return true;
+    }
+    return false;
+  };
+  auto table_full = [&]() -> int { return groups_now() > K.aux[0].agg.group_limit || pairs_over() ? 1 : 0; };
   auto defer_rest = [&](int64_t from) {                   // uniform across the CTA
     if (from >= n_pos) return;
     const AggParams& A = K.aux[0].agg;
@@ -1826,7 +1862,8 @@ __global__ void __launch_bounds__(NT, MINB) pipeline_kernel(const __grid_constan
     }
     // the group count is read at the top of the tile and only looked at before barrier (B): its latency is hidden
     unsigned long long g_now = 0;
-    if (guarded && threadIdx.x == 0) g_now = groups_now();
+    bool p_over = false;
+    if (guarded && threadIdx.x == 0) { g_now = groups_now(); p_over = pairs_over(); }
     const bool prefetched = n_stages == 2 && nxt < n_end && !defer;
     if (prefetched) issue(dynamic ? nxt : tile_of(nxt), s ^ 1);   // prefetch while this tile is computed (consumed after barrier B)
     const int64_t cur_tile = dynamic ? cur : tile_of(cur);
@@ -1850,7 +1887,7 @@ __global__ void __launch_bounds__(NT, MINB) pipeline_kernel(const __grid_constan
         default: break;
       }
     }
-    if (guarded && threadIdx.x == 0) sm->defer[(it + 1) & 1] = g_now > K.aux[0].agg.group_limit ? 1 : 0;
+    if (guarded && threadIdx.x == 0) sm->defer[(it + 1) & 1] = g_now > K.aux[0].agg.group_limit || p_over ? 1 : 0;
     if (KC == KC_OTHER && P.sink == SINK_BUILD && threadIdx.x == 0) sm->defer[(it + 1) & 1] = sm->cache_count > CHAIN_CACHE_ENTRIES / 2 ? 1 : 0;
     __syncthreads();                                          // (B) stage s and scratch are free again
     if (KC == KC_OTHER && P.sink == SINK_BUILD && sm->defer[(it + 1) & 1]) {      // crowded cache: push everything, start over

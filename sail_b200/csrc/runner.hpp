@@ -33,7 +33,7 @@ inline bool timing_enabled() { static const bool on = getenv("SAILGPU_TIMING") !
 inline void dump_pipeline(const CompiledPipeline& cp) {
   static const char* names[] = {"NOP", "UNPACK_BITS", "CONST", "MOV", "CVT", "ADD", "SUB", "MUL", "DIV", "REM", "NEG", "MULW", "MUL128_64", "DIVROUND",
                                 "EQ", "NE", "LT", "LE", "GT", "GE", "AND", "OR", "NOT", "ANDNOT", "SELECT", "STR_EQ_LONG", "STR_LIKE", "DATE_PART", "PROBE", "GATHER", "SUBSTR",
-                                "TS_PART", "TS_TRUNC", "MUL_POW10_CHK", "CHAR_LEN"};
+                                "TS_PART", "TS_TRUNC", "MUL_POW10_CHK", "CHAR_LEN", "DISTINCT_FIRST"};
   static const char* sinks[] = {"STORE", "COMPACT", "AGG", "BUILD", "PARTITION"};
   fprintf(stderr, "[sailgpu pipeline] sink=%s rows/thread=%d stages=%d smem=%zu B (temps %u, stage %u, hot %u) inputs=%zu outs=%zu%s\n",
           cp.sink >= 0 && cp.sink < 5 ? sinks[cp.sink] : "?", cp.rpt, cp.n_stages, cp.smem_bytes, cp.temps_bytes, cp.stage_bytes, cp.hot_bytes,
@@ -73,6 +73,10 @@ struct PipelineRunner {
   int hot_wanted = 8;
   int64_t rows_seen = 0;                 // rows launched through this runner (specialisation threshold)
   uint64_t group_limit_cap = ~0ull;      // bounded aggregation: extra cap on the launch's group limit (see PipelineOp)
+  // bounded aggregation: the limits the last guarded launch ran with (group table, pair sets), so the host can tell which
+  // table a hand-back was for
+  uint64_t last_group_limit = ~0ull, last_pair_limit[MAX_DISTINCT] = {};
+  BufPtr distinct_params;                // device copy of the pair-set descriptors of both stages (PipelineAux::distinct)
   std::function<void(PipelineCompiler&, CompiledPipeline&)> custom_sink;   // build / partition sinks
   std::function<void(PipelineCompiler&, CompiledPipeline&)> pre_stages;    // probe ops injected before the stages
 
@@ -178,6 +182,8 @@ struct PipelineRunner {
     P.prog = nullptr;
     auto K = std::make_unique<KernelArgs>();
     memset(K.get(), 0, sizeof(KernelArgs));
+    const int n_distinct = aux_host ? aux_host->n_distinct : 0;
+    std::vector<AggParams> dist(n_distinct ? (size_t)(2 * MAX_DISTINCT) : 0);
     for (int st = 0; st < 2; ++st) {
       const uint32_t add = (uint32_t)st * cp->stage_bytes;
       PipelineParams& Q = K->P[st];
@@ -204,6 +210,11 @@ struct PipelineRunner {
           for (int i = 0; i < A.probe[q].n_keys; ++i) rs_key(A.probe[q].keys[i], add);
           A.probe[q].rowid_slot = rs(A.probe[q].rowid_slot, add);
           A.probe[q].match_slot = rs(A.probe[q].match_slot, add);
+        }
+        for (int d = 0; d < n_distinct; ++d) {      // aux_host->distinct: the host copy of the descriptors
+          AggParams& D = dist[(size_t)(st * MAX_DISTINCT + d)];
+          D = aux_host->distinct[d];
+          for (int i = 0; i < D.n_keys; ++i) rs_key(D.keys[i], add);
         }
       }
     }
@@ -244,7 +255,20 @@ struct PipelineRunner {
       const uint64_t slack = std::min<uint64_t>(in_flight * (uint64_t)grid * (uint64_t)P.tile_rows, (uint64_t)P.n_rows) + (uint64_t)grid * (uint64_t)std::max(0, cp->agg.hot_groups);
       const uint64_t limit = std::min<uint64_t>(cap / 2 > slack ? cap / 2 - slack : 0, group_limit_cap);
       for (int st = 0; st < 2; ++st)
-        if (K->aux[st].agg.group_limit == ~0ull) K->aux[st].agg.group_limit = limit;
+        if (K->aux[st].agg.group_limit == ~0ull && cp->agg.n_keys > 0) K->aux[st].agg.group_limit = limit;     // one group never grows
+      // a pair set gains at most one pair per row: only the rows in flight count
+      const uint64_t pair_slack = std::min<uint64_t>(in_flight * (uint64_t)grid * (uint64_t)P.tile_rows, (uint64_t)P.n_rows);
+      for (int d = 0; d < n_distinct; ++d) {
+        const uint64_t dcap = dist[(size_t)d].capacity_mask + 1;
+        last_pair_limit[d] = dcap / 2 > pair_slack ? dcap / 2 - pair_slack : 0;
+        for (int st = 0; st < 2; ++st) dist[(size_t)(st * MAX_DISTINCT + d)].group_limit = last_pair_limit[d];
+      }
+      last_group_limit = K->aux[0].agg.group_limit;
+    }
+    if (n_distinct) {
+      if (!distinct_params) distinct_params = dev_alloc(ctx, dist.size() * sizeof(AggParams));
+      SG_CUDA(cudaMemcpyAsync(distinct_params->ptr, dist.data(), dist.size() * sizeof(AggParams), cudaMemcpyHostToDevice, ctx->stream));
+      for (int st = 0; st < 2; ++st) K->aux[st].distinct = static_cast<const AggParams*>(distinct_params->ptr) + st * MAX_DISTINCT;
     }
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     const bool timed = timing_enabled();

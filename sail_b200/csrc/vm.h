@@ -24,6 +24,7 @@ constexpr int MAX_KEYS = 6;
 constexpr int MAX_KEY_WORDS = 8;   // 64 bytes of packed key
 constexpr int MAX_ACCS = 16;
 constexpr int MAX_PROBES = 4;
+constexpr int MAX_DISTINCT = 4;    // pair sets (distinct arguments) of one aggregate
 constexpr int REG_GROUPS = 4;      // hot groups held in registers by the integer fast path
 constexpr int REG_ACCS = 6;        // accumulators held in registers per group
 constexpr int HOT_KEY_WORDS = 4;   // group keys wider than 32 bytes skip the hot paths (global table only)
@@ -58,6 +59,8 @@ enum VmBase : uint16_t {
   OP_MUL_POW10_CHK, // dst(I128) <- a(I128) * imm (a power of ten); ERR_OVERFLOW when a row of c (rows evaluated, or NO_SLOT
                     //   for all) leaves i128: the decimal division rescale that can overflow
   OP_CHAR_LEN,      // dst(I32) <- character_length(view a): UTF-8 characters
+  OP_DISTINCT_FIRST,// dst(B) <- the row is active (c: mask slot or NO_SLOT), its DISTINCT argument is valid, and this row claimed
+                    //   its (group key, argument) pair in pair set aux (PipelineAux::distinct): true on one row per pair
   OP_COUNT_
 };
 // OP_TS_PART / OP_TS_TRUNC parts.  TS_SECOND: the part is the microsecond within the minute, the truncation the whole second;
@@ -238,6 +241,11 @@ struct PipelineAux {
   BuildParams build;
   PartitionParams part;
   ProbeParams probe[MAX_PROBES];
+  // DISTINCT aggregates: one pair set per distinct argument -- a group table without accumulators whose key is the group key
+  // (always with a null-mask word) followed by the argument.  The descriptors live in device memory (this stage's
+  // MAX_DISTINCT entries), so that pipelines without DISTINCT launch with the parameter block they had.
+  const AggParams* distinct;
+  int32_t n_distinct;
 };
 
 // Everything uniform across the grid travels as ONE kernel parameter (constant bank: uniform loads,

@@ -98,7 +98,8 @@ def project(child: Node, exprs: list) -> Node:
 
 
 def aggregate(child: Node, mode: str, group_by: list, aggs: list) -> Node:
-    """group_by: column names or (expr, name); aggs: (fn, arg_expr|None, name, input_type)"""
+    """group_by: column names or (expr, name); aggs: (fn, arg_expr|None, name, input_type), or (fn, arg, name, input_type, True)
+    for fn(DISTINCT arg)"""
     gb = []
     for g in group_by:
         if isinstance(g, str):
@@ -106,10 +107,12 @@ def aggregate(child: Node, mode: str, group_by: list, aggs: list) -> Node:
         gb.append({"expr": resolve(g[0], child.names), "name": g[1]})
     merging = mode in ("final", "final_partitioned")
     specs, names = [], [g["name"] for g in gb]
-    for fn, arg, name, in_type in aggs:
+    for fn, arg, name, in_type, *distinct in aggs:
         a = {"fn": fn, "name": name, "input_type": in_type}
         if not merging:
             a["args"] = [] if arg is None else [resolve(arg, child.names)]
+        if distinct and distinct[0]:
+            a["distinct"] = True
         specs.append(a)
         if mode == "partial":
             names += [f"{name}[count]", f"{name}[sum]"] if fn == "avg" else [f"{name}[{fn}]"]

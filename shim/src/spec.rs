@@ -130,14 +130,20 @@ pub fn aggregate(a: &AggregateExec) -> Option<Value> {
     let merging = matches!(a.mode(), AggregateMode::Final | AggregateMode::FinalPartitioned);
     let mut aggs = vec![];
     for f in a.aggr_expr() {
-        if f.is_distinct() || !f.order_bys().is_empty() { return None; }
+        if !f.order_bys().is_empty() { return None; }
         let fun = f.fun().name().to_lowercase();
         if !matches!(fun.as_str(), "sum" | "avg" | "count" | "min" | "max") { return None; }
+        // DISTINCT over one argument of a single-mode aggregate; in a partial / final pair its state is a List column, and such
+        // a pair stays a DataFusion node
+        let distinct = f.is_distinct();
+        let single = matches!(a.mode(), AggregateMode::Single | AggregateMode::SinglePartitioned);
+        if distinct && (!single || f.expressions().len() != 1) { return None; }
         let args: Option<Vec<Value>> = f.expressions().iter().map(expr).collect();
         // input_type: type of the argument BEFORE aggregation (the final phases only see the state columns)
         let in_t = f.expressions().first().and_then(|e| e.data_type(&a.input_schema()).ok()).and_then(|t| type_name(&t));
         let mut j = json!({"fn": fun, "name": f.name(), "input_type": in_t});
-        if !merging { j["args"] = Value::Array(if fun == "count" && is_count_star(f) { vec![] } else { args? }); }
+        if !merging { j["args"] = Value::Array(if fun == "count" && !distinct && is_count_star(f) { vec![] } else { args? }); }
+        if distinct { j["distinct"] = json!(true); }
         aggs.push(j);
     }
     Some(json!({"op": "aggregate", "mode": mode, "group_by": group_by?, "aggs": aggs}))
