@@ -850,6 +850,18 @@ std::unique_ptr<Op> make_nlj_op(Ctx* ctx, const Json& spec, const std::vector<Sc
 // ================================================================================================
 // SortExec (+ TopK)
 // ================================================================================================
+// scratch of radix_sort_indices for n rows; `hold` keeps its buffers
+static RadixScratch radix_scratch(Ctx* ctx, int64_t n, std::vector<BufPtr>& hold) {
+  const int64_t n_chunks = (n + 2047) / 2048;
+  auto buf = [&](size_t bytes) { hold.push_back(dev_alloc(ctx, bytes)); return hold.back()->ptr; };
+  RadixScratch S;
+  S.idx_a = static_cast<uint32_t*>(buf((size_t)n * 4)); S.idx_b = static_cast<uint32_t*>(buf((size_t)n * 4));
+  S.kw_a = static_cast<uint64_t*>(buf((size_t)n * 8)); S.kw_b = static_cast<uint64_t*>(buf((size_t)n * 8));
+  S.hist = static_cast<uint32_t*>(buf((size_t)n_chunks * 256 * 4)); S.offs = static_cast<uint64_t*>(buf((size_t)n_chunks * 256 * 8));
+  S.scan_scratch = static_cast<uint64_t*>(buf(1026 * 8));
+  return S;
+}
+
 struct SortOp : Op {
   struct Key { ExprPtr e; bool asc, nulls_first; };
   std::vector<Key> keys;
@@ -876,9 +888,9 @@ struct SortOp : Op {
     return false;
   }
 
-  struct Encoded { BufPtr keys, bits; int key_bytes = 0; };
+  struct Encoded { BufPtr keys, bits; int key_bytes = 0; std::vector<BufPtr> ranks; };
 
-  // the key columns of every row as the encoder and the small sort read them (string keys: no length bound yet)
+  // the key columns of every row as the encoder, the small sort and the TopK selection read them (string keys: no ranks yet)
   SortEncodeParams describe_keys(const BatchPtr& all, const Schema& sch, const std::vector<Key>& ks) {
     SortEncodeParams E; memset(&E, 0, sizeof(E));
     E.n = all->rows; E.n_keys = (int)ks.size();
@@ -891,7 +903,7 @@ struct SortOp : Op {
       s.data = static_cast<const uint8_t*>(c.data->ptr);
       s.validity_bits = c.validity ? static_cast<const uint8_t*>(c.validity->ptr) : nullptr;
       s.asc = ks[k].asc; s.nulls_first = ks[k].nulls_first;
-      if (t.is_string()) { s.kind = SORT_VIEW; s.width = 16; }
+      if (t.is_string()) { s.kind = SORT_VIEW; s.width = 16; s.enc_bytes = 4; }
       else if (t.id == TypeId::Bool) { s.kind = SORT_BOOL; s.width = 1; s.enc_bytes = 1; }
       else if (t.is_float()) { SG_CHECK(t.id == TypeId::Float64, SAILGPU_ERR_UNSUPPORTED, "Float32 sort keys"); s.kind = SORT_F64; s.width = 8; s.enc_bytes = 8; }
       else if (t.is_unsigned_int()) { s.kind = SORT_UINT; s.width = t.arrow_width(); s.enc_bytes = s.width; }
@@ -900,27 +912,38 @@ struct SortOp : Op {
     return E;
   }
 
-  // order-preserving fixed-width encoding of the sort keys of every row (memcmp order == requested order)
+  // the dense rank of every row's string in a string key column (string_ranks, relational.cu)
+  BufPtr string_ranks_of(const SortKeyCol& c, int64_t n) {
+    std::vector<BufPtr> hold;
+    auto buf = [&](size_t bytes) { hold.push_back(dev_alloc(ctx, bytes)); return hold.back()->ptr; };
+    StringRankScratch S;
+    S.radix = radix_scratch(ctx, n, hold);
+    S.keys = static_cast<uint8_t*>(buf((size_t)n * 13));
+    S.perm = static_cast<uint32_t*>(buf((size_t)n * 4)); S.head = static_cast<uint32_t*>(buf((size_t)n * 4)); S.rowof = static_cast<uint32_t*>(buf((size_t)n * 4));
+    for (int i = 0; i < 2; ++i) { S.opos[i] = static_cast<uint32_t*>(buf((size_t)n * 4)); S.grp[i] = static_cast<uint32_t*>(buf((size_t)n * 4)); }
+    S.flags = static_cast<uint64_t*>(buf((size_t)n * 8)); S.before = static_cast<uint64_t*>(buf((size_t)n * 8));
+    S.scan_scratch = static_cast<uint64_t*>(buf(1026 * 8));
+    S.ctrl = static_cast<uint32_t*>(buf(32 * 4));
+    BufPtr rank = dev_alloc(ctx, (size_t)n * 4);
+    int launches = 0, syncs = 0;
+    SG_CUDA(string_ranks(c.data, c.validity_bits, n, static_cast<uint32_t*>(rank->ptr), S, ctx->stream, &launches, &syncs));
+    m.kernel_launches += (uint64_t)launches;
+    ctx->host_syncs += (uint64_t)syncs;
+    return rank;
+  }
+
+  // order-preserving fixed-width encoding of the sort keys of every row (memcmp order == requested order).  A string key is its
+  // null byte and its 4-byte dense rank among the rows, so the width does not depend on the strings' lengths.
   Encoded encode_keys(const BatchPtr& all, const Schema& sch, const std::vector<Key>& ks) {
     const int64_t n = all->rows;
     SortEncodeParams E = describe_keys(all, sch, ks);
-    int off = 0;
-    BufPtr maxlen = dev_alloc_zero(ctx, 8 * 8);
-    std::vector<int> str_keys;
-    for (size_t k = 0; k < ks.size(); ++k)
-      if (E.cols[k].kind == SORT_VIEW) { SG_CUDA(launch_max_view_len(E.cols[k].data, n, static_cast<unsigned int*>(maxlen->ptr) + k, ctx->stream)); str_keys.push_back((int)k); }
-    if (!str_keys.empty()) {
-      unsigned int lens[8] = {0};
-      SG_CUDA(cudaMemcpyAsync(lens, maxlen->ptr, sizeof(lens), cudaMemcpyDeviceToHost, ctx->stream));
-      stream_sync(ctx);
-      for (int k : str_keys) {
-        SG_CHECK(lens[k] <= 256, SAILGPU_ERR_UNSUPPORTED, "sort key strings longer than 256 bytes are not supported yet");
-        E.cols[k].str_len = (int)lens[k]; E.cols[k].enc_bytes = (int)lens[k] + 4;
-      }
-    }
-    for (size_t k = 0; k < ks.size(); ++k) { E.cols[k].out_off = off; off += 1 + E.cols[k].enc_bytes; }
-    E.key_bytes = off;
     Encoded out;
+    int off = 0;
+    for (size_t k = 0; k < ks.size(); ++k) {
+      if (E.cols[k].kind == SORT_VIEW) { out.ranks.push_back(string_ranks_of(E.cols[k], n)); E.cols[k].rank = static_cast<const uint32_t*>(out.ranks.back()->ptr); }
+      E.cols[k].out_off = off; off += 1 + E.cols[k].enc_bytes;
+    }
+    E.key_bytes = off;
     out.key_bytes = off;
     out.keys = dev_alloc(ctx, (size_t)n * off);
     out.bits = dev_alloc_zero(ctx, (size_t)off * 8);
@@ -957,30 +980,31 @@ struct SortOp : Op {
       return take_rows(all, sch, static_cast<const int64_t*>(idx->ptr), take);
     }
     Encoded enc = encode_keys(all, sch, ks);
-    const int64_t n_chunks = (n + 2047) / 2048;
-    BufPtr ia = dev_alloc(ctx, (size_t)n * 4), ib = dev_alloc(ctx, (size_t)n * 4), ka = dev_alloc(ctx, (size_t)n * 8), kbuf = dev_alloc(ctx, (size_t)n * 8),
-           hist = dev_alloc(ctx, (size_t)n_chunks * 256 * 4), offs = dev_alloc(ctx, (size_t)n_chunks * 256 * 8), scr = dev_alloc(ctx, 1026 * 8);
-    RadixScratch S;
-    S.idx_a = static_cast<uint32_t*>(ia->ptr); S.idx_b = static_cast<uint32_t*>(ib->ptr);
-    S.kw_a = static_cast<uint64_t*>(ka->ptr); S.kw_b = static_cast<uint64_t*>(kbuf->ptr);
-    S.hist = static_cast<uint32_t*>(hist->ptr); S.offs = static_cast<uint64_t*>(offs->ptr); S.scan_scratch = static_cast<uint64_t*>(scr->ptr);
+    std::vector<BufPtr> hold;
+    const RadixScratch S = radix_scratch(ctx, n, hold);
     int sort_launches = 0;
     SG_CUDA(radix_sort_indices(static_cast<const uint8_t*>(enc.keys->ptr), enc.key_bytes, n, S, static_cast<const uint32_t*>(enc.bits->ptr), ctx->stream, &sort_launches));
     m.kernel_launches += (uint64_t)(sort_launches + 1);
     BufPtr idx = dev_alloc(ctx, (size_t)take * 8);
-    SG_CUDA(launch_widen_u32(static_cast<const uint32_t*>(ia->ptr), static_cast<int64_t*>(idx->ptr), take, ctx->stream));
+    SG_CUDA(launch_widen_u32(S.idx_a, static_cast<int64_t*>(idx->ptr), take, ctx->stream));
     return take_rows(all, sch, static_cast<const int64_t*>(idx->ptr), take);
   }
 
-  // TopK: radix-select the rows that can be among the first `k` on the leading 8 key bytes (one 8 B/row pass per 11 bits),
-  // then sort only those.  The candidates carry their row number as a last key, so ties come out in input order exactly as
-  // the (stable) full sort would deliver them.  Returns null when the selection does not narrow the input enough.
+  // TopK: radix-select the rows that can be among the first `k` on a word that holds the leading 8 bytes of the encoded key,
+  // a string key's leading bytes in place of its rank (one 8 B/row pass per 11 bits), then sort only those.  The candidates
+  // carry their row number as a last key, so ties come out in input order exactly as the (stable) full sort would deliver them.
+  // Returns null when the selection does not narrow the input enough.
   static constexpr int64_t TOPK_MIN_ROWS = 1 << 18, TOPK_MAX_K = 1 << 16;
   BatchPtr topk_rows(const BatchPtr& all, const Schema& sch, const std::vector<Key>& ks, int64_t k) {
     const int64_t n = all->rows;
-    Encoded enc = encode_keys(all, sch, ks);
-    const uint8_t* kp = static_cast<const uint8_t*>(enc.keys->ptr);
-    const int total_bits = std::min(64, enc.key_bytes * 8);
+    const SortEncodeParams E = describe_keys(all, sch, ks);
+    int word_bytes = 0;         // bytes of the word that are not constant zero: nothing follows a string key
+    for (int i = 0; i < E.n_keys && word_bytes < 8; ++i) word_bytes += E.cols[i].kind == SORT_VIEW ? 8 : 1 + E.cols[i].enc_bytes;
+    const int total_bits = std::min(64, word_bytes * 8);
+    BufPtr words = dev_alloc(ctx, (size_t)n * 8);
+    const uint64_t* kp = static_cast<const uint64_t*>(words->ptr);
+    SG_CUDA(launch_topk_words(E, static_cast<uint64_t*>(words->ptr), ctx->stream));
+    m.kernel_launches += 1;
     const int64_t want_at_most = std::max<int64_t>(4 * k, 1 << 16);
     BufPtr hist = dev_alloc(ctx, 2048 * 4);
     std::vector<uint32_t> h(2048);
@@ -990,7 +1014,7 @@ struct SortOp : Op {
     while (used < total_bits && below + cand > want_at_most) {
       const int db = std::min(11, total_bits - used);
       SG_CUDA(cudaMemsetAsync(hist->ptr, 0, 2048 * 4, ctx->stream));
-      SG_CUDA(launch_topk_hist(kp, enc.key_bytes, n, used, prefix, db, static_cast<uint32_t*>(hist->ptr), ctx->stream));
+      SG_CUDA(launch_topk_hist(kp, n, used, prefix, db, static_cast<uint32_t*>(hist->ptr), ctx->stream));
       SG_CUDA(cudaMemcpyAsync(h.data(), hist->ptr, 2048 * 4, cudaMemcpyDeviceToHost, ctx->stream));
       stream_sync(ctx);
       m.kernel_launches += 1;
@@ -1004,7 +1028,7 @@ struct SortOp : Op {
     }
     if (below + cand > std::max<int64_t>(want_at_most, n / 4)) return nullptr;       // heavy ties on the leading bytes: sort everything
     BufPtr idx = dev_alloc(ctx, (size_t)(below + cand) * 8), ctr = dev_alloc_zero(ctx, 8);
-    SG_CUDA(launch_topk_compact(kp, enc.key_bytes, n, used, prefix, static_cast<int64_t*>(idx->ptr), static_cast<unsigned long long*>(ctr->ptr), ctx->stream));
+    SG_CUDA(launch_topk_compact(kp, n, used, prefix, static_cast<int64_t*>(idx->ptr), static_cast<unsigned long long*>(ctr->ptr), ctx->stream));
     m.kernel_launches += 1;
     const int64_t nc = below + cand;
     BatchPtr sub = take_rows(all, sch, static_cast<const int64_t*>(idx->ptr), nc);
@@ -1213,37 +1237,32 @@ struct WideAggOp : Op {
     for (size_t i = 0; i < gb.a.size(); ++i) kex.push_back(jobj({{"expr", gb.a[i].at("expr")}, {"name", jstr("__k" + std::to_string(i))}}));
     Schema ks;
     BatchPtr kb = through(jobj({{"op", jstr("projection")}, {"exprs", jarr(kex)}}), in, all, &ks);
-    // 2. rows in key order
+    // 2. rows with equal keys next to each other: ordered by a 64-bit hash of the key columns (8 radix digits whatever the key
+    //    width); only if two different keys share a hash -- equal keys would then not be adjacent -- by the sort encoding
     SortOp so; so.ctx = ctx;
     std::vector<SortOp::Key> keys;
     for (int i = 0; i < n_keys; ++i) keys.push_back({parse_expr(jcol(i), ks), true, true});
-    SortOp::Encoded enc = so.encode_keys(kb, ks, keys);
-    const int64_t n_chunks = (n + 2047) / 2048;
-    BufPtr ia = dev_alloc(ctx, (size_t)n * 4), ib = dev_alloc(ctx, (size_t)n * 4), ka = dev_alloc(ctx, (size_t)n * 8), kbuf = dev_alloc(ctx, (size_t)n * 8),
-           hist = dev_alloc(ctx, (size_t)n_chunks * 256 * 4), offs = dev_alloc(ctx, (size_t)n_chunks * 256 * 8), scr = dev_alloc(ctx, 1026 * 8);
-    RadixScratch S;
-    S.idx_a = static_cast<uint32_t*>(ia->ptr); S.idx_b = static_cast<uint32_t*>(ib->ptr);
-    S.kw_a = static_cast<uint64_t*>(ka->ptr); S.kw_b = static_cast<uint64_t*>(kbuf->ptr);
-    S.hist = static_cast<uint32_t*>(hist->ptr); S.offs = static_cast<uint64_t*>(offs->ptr); S.scan_scratch = static_cast<uint64_t*>(scr->ptr);
-    // rows with equal keys next to each other: ordered by a 64-bit hash of the encoded key (8 radix digits whatever the key
-    // width); only if two different keys share a hash -- equal keys would then not be adjacent -- by the full key
+    const SortEncodeParams E = so.describe_keys(kb, ks, keys);
+    std::vector<BufPtr> hold;
+    const RadixScratch S = radix_scratch(ctx, n, hold);
     int sort_launches = 0;
     BufPtr hk = dev_alloc(ctx, (size_t)n * 8), all_bits = dev_alloc(ctx, 16 * 4), coll = dev_alloc_zero(ctx, 8);
     SG_CUDA(cudaMemsetAsync(all_bits->ptr, 0xFF, 16 * 4, ctx->stream));
-    SG_CUDA(launch_key_hash(static_cast<const uint8_t*>(enc.keys->ptr), enc.key_bytes, n, static_cast<uint8_t*>(hk->ptr), ctx->stream));
+    SG_CUDA(launch_group_hash(E, static_cast<uint8_t*>(hk->ptr), ctx->stream));
     SG_CUDA(radix_sort_indices(static_cast<const uint8_t*>(hk->ptr), 8, n, S, static_cast<const uint32_t*>(all_bits->ptr), ctx->stream, &sort_launches));
     // 3. runs of equal keys -> dense group numbers, one representative row per group
     BufPtr heads = dev_alloc(ctx, (size_t)n * 4), before = dev_alloc(ctx, (size_t)n * 8), scr2 = dev_alloc(ctx, 1026 * 8);
-    SG_CUDA(launch_group_heads(static_cast<const uint8_t*>(enc.keys->ptr), enc.key_bytes, S.idx_a, n, static_cast<uint32_t*>(heads->ptr),
-                               static_cast<const uint8_t*>(hk->ptr), static_cast<unsigned long long*>(coll->ptr), ctx->stream));
+    SG_CUDA(launch_group_heads(E, S.idx_a, static_cast<uint32_t*>(heads->ptr), static_cast<const uint8_t*>(hk->ptr), static_cast<unsigned long long*>(coll->ptr),
+                               ctx->stream));
     unsigned long long n_coll = 0;
     SG_CUDA(cudaMemcpyAsync(&n_coll, coll->ptr, 8, cudaMemcpyDeviceToHost, ctx->stream));
     stream_sync(ctx);
     if (n_coll != 0 || getenv("SAILGPU_WIDEAGG_FULL_SORT") != nullptr) {
       int more = 0;
+      SortOp::Encoded enc = so.encode_keys(kb, ks, keys);
       SG_CUDA(radix_sort_indices(static_cast<const uint8_t*>(enc.keys->ptr), enc.key_bytes, n, S, static_cast<const uint32_t*>(enc.bits->ptr), ctx->stream, &more));
-      SG_CUDA(launch_group_heads(static_cast<const uint8_t*>(enc.keys->ptr), enc.key_bytes, S.idx_a, n, static_cast<uint32_t*>(heads->ptr), nullptr, nullptr, ctx->stream));
-      sort_launches += more + 1;
+      SG_CUDA(launch_group_heads(E, S.idx_a, static_cast<uint32_t*>(heads->ptr), nullptr, nullptr, ctx->stream));
+      sort_launches += more + 1 + (int)so.m.kernel_launches;
     }
     SG_CUDA(launch_exclusive_scan_u32(static_cast<const uint32_t*>(heads->ptr), n, static_cast<uint64_t*>(before->ptr), static_cast<uint64_t*>(scr2->ptr), ctx->stream));
     uint64_t n_groups = 0;

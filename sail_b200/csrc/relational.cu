@@ -4,9 +4,11 @@
 //     walk the open-addressing run, count then emit (build row, probe row) pairs.  The unique-key
 //     fast path never comes here: it runs inside the tile pipeline (OP_PROBE, pipeline.cu).
 //   * sort_encode + radix passes : SortExec.  Rows are encoded into order-preserving fixed-width keys
-//     (arrow-row style: null byte, sign-flipped big-endian integers, IEEE total order, padded strings
-//     + length) and sorted by a stable LSD radix sort on 8-bit digits whose per-warp ranking uses
+//     (arrow-row style: null byte, sign-flipped big-endian integers, IEEE total order, strings as their
+//     dense rank) and sorted by a stable LSD radix sort on 8-bit digits whose per-warp ranking uses
 //     __match_any_sync / ballots ("radix sort via warp shuffles", BASELINE.json north_star).
+//   * string_ranks : the dense memcmp-order rank of every string of a column, by MSD refinement of
+//     8-byte windows, so that a string key encodes in 4 bytes whatever its length.
 //   * gather_rows : `take` of fixed-width / view columns by row index.
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -195,13 +197,9 @@ __global__ void sort_encode_kernel(SortEncodeParams P) {
           SG_PUT(o, v ^ inv);
           break;
         }
-        default: {            // SORT_VIEW: bytes padded with zeros to c.str_len, then 4-byte big-endian length
-          const uint8_t* vp = c.data + i * 16;
-          const ulonglong2 v = *reinterpret_cast<const ulonglong2*>(vp);
-          const uint32_t len = (uint32_t)v.x;
-          const uint8_t* s = view_ptr(v, vp);
-          for (int b = 0; b < c.str_len; ++b) SG_PUT(o + b, ((uint32_t)b < len ? s[b] : 0) ^ inv);
-          for (int b = 0; b < 4; ++b) SG_PUT(o + c.str_len + b, (uint8_t)(len >> (24 - 8 * b)) ^ inv);
+        default: {            // SORT_VIEW: the string's dense rank (launch_string_ranks), 4 bytes big-endian
+          const uint32_t r = c.rank[i];
+          for (int b = 0; b < 4; ++b) SG_PUT(o + b, (uint8_t)(r >> (24 - 8 * b)) ^ inv);
         }
       }
     }
@@ -362,15 +360,24 @@ cudaError_t launch_small_sort_cols(const SortEncodeParams& P, uint32_t* idx_out,
 // Sorts row indices by the encoded keys; `S.idx_a` receives the final order.  `bits` = the [2 * key_bytes] words
 // sort_encode_kernel filled.  Synchronises the stream once (to read `bits`).  *launches counts the kernels issued.
 cudaError_t radix_sort_indices(const uint8_t* keys, int key_bytes, int64_t n, const RadixScratch& S, const uint32_t* bits, cudaStream_t s, int* launches) {
+  if (launches) *launches = 0;
+  if (n == 0) return cudaSuccess;
+  std::vector<uint32_t> hb((size_t)key_bytes * 2);
+  if (n > 1024) {
+    cudaError_t e = cudaMemcpyAsync(hb.data(), bits, hb.size() * 4, cudaMemcpyDeviceToHost, s);
+    if (e != cudaSuccess) return e;
+    e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) return e;
+  }
+  return radix_sort_indices_host_bits(keys, key_bytes, n, S, hb.data(), s, launches);
+}
+// the same with `hb` = those words already on the host: no synchronisation
+cudaError_t radix_sort_indices_host_bits(const uint8_t* keys, int key_bytes, int64_t n, const RadixScratch& S, const uint32_t* hb, cudaStream_t s, int* launches) {
   int nl = 0;
   if (launches) *launches = 0;
   if (n == 0) return cudaSuccess;
   if (n <= 1024) { small_sort_kernel<<<1, 1024, 0, s>>>(keys, key_bytes, (int)n, S.idx_a); if (launches) *launches = 1; return cudaGetLastError(); }
-  std::vector<uint32_t> hb((size_t)key_bytes * 2);
-  cudaError_t e = cudaMemcpyAsync(hb.data(), bits, hb.size() * 4, cudaMemcpyDeviceToHost, s);
-  if (e != cudaSuccess) return e;
-  e = cudaStreamSynchronize(s);
-  if (e != cudaSuccess) return e;
+  cudaError_t e = cudaSuccess;
   auto trivial = [&](int d) { return (hb[(size_t)d] & hb[(size_t)key_bytes + d] & 0xFFu) == 0; };
   const int64_t n_chunks = (n + RADIX_CHUNK - 1) / RADIX_CHUNK;
   const int blocks = (int)((n_chunks + 7) / 8);
@@ -406,31 +413,201 @@ cudaError_t radix_sort_indices(const uint8_t* keys, int key_bytes, int64_t n, co
 }
 
 // ------------------------------------------------------------------------------------------------
-// TopK selection (SortExec with fetch = k, test_tpch.plan.yaml:27,79; ClickBench ORDER BY .. LIMIT 10): radix SELECT on
-// the leading 8 bytes of the encoded key instead of sorting all n rows.  One level = one streaming pass over 8 B/row:
-// histogram of the next 11 bits among the rows whose consumed prefix equals the threshold path.
+// string ranks: the dense rank of every string of a Utf8View column in memcmp order (a proper prefix before its extensions).
+// MSD refinement: round r orders the rows of every open group by (group, the 8 bytes of the string at 8r big-endian and
+// zero-padded, marker = min(bytes left, 9)) with the radix sort above and writes them back into their group's positions.
+// A group is open while it has two or more rows and its strings go on past the window (marker 9).  A row leaves as soon as
+// its group is settled: it pays for the windows it shares with another row, not for the longest string of the column.
+// Null rows rank as the empty string (the encoding's null byte decides their place).
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint64_t key_word_be(const uint8_t* k, int key_bytes) {      // first 8 key bytes as a big-endian number (zero padded)
-  uint64_t w = 0;
-  const int nb = key_bytes < 8 ? key_bytes : 8;
-  for (int b = 0; b < nb; ++b) w |= (uint64_t)k[b] << (56 - 8 * b);
-  return w;
+constexpr int RANK_KEY = 13;          // 4 B group, 8 B window, 1 B marker
+constexpr uint32_t RANK_WIN = 8;
+
+__device__ __forceinline__ void rank_bits_put(uint32_t* bits, int pos, uint32_t o, uint32_t a) {
+  if (o) atomicOr(bits + pos, o);
+  if (a != 0xFFu) atomicOr(bits + RANK_KEY + pos, a ^ 0xFFu);
 }
-__global__ void topk_hist_kernel(const uint8_t* __restrict__ keys, int key_bytes, int64_t n, int used, uint64_t prefix, int digit_bits, uint32_t* __restrict__ hist) {
+// the round's key of every open row (count ? *count : n of them); records which key bits vary, as sort_encode_kernel does
+__global__ void rank_encode_kernel(const uint8_t* __restrict__ views, const uint8_t* __restrict__ validity, int64_t n, const uint32_t* __restrict__ count,
+                                   uint32_t offset, const uint32_t* __restrict__ opos, const uint32_t* __restrict__ grp, const uint32_t* __restrict__ perm,
+                                   uint32_t* __restrict__ rowof, uint8_t* __restrict__ keys, uint32_t* __restrict__ bits) {
+  const int64_t m = count ? (int64_t)*count : n;
+  uint32_t og = 0, ag = 0xFFFFFFFFu, om = 0, am = 0xFFu;
+  uint64_t ow = 0, aw = ~0ull;
+  for (int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; j < m; j += (int64_t)gridDim.x * blockDim.x) {
+    const uint32_t row = opos ? perm[opos[j]] : (uint32_t)j;
+    if (opos) rowof[j] = row;
+    const uint32_t g = grp ? grp[j] : 0u;
+    const uint8_t* vp = views + (int64_t)row * 16;
+    const ulonglong2 v = *reinterpret_cast<const ulonglong2*>(vp);
+    const bool valid = !validity || ((validity[row >> 3] >> (row & 7)) & 1);
+    const uint32_t rest = (valid ? (uint32_t)v.x : 0u) - offset;       // the rows of an open group go on past `offset`
+    const uint8_t* sp = view_ptr(v, vp) + offset;
+    const uint32_t nb = rest < RANK_WIN ? rest : RANK_WIN;
+    uint64_t w = 0;
+    for (uint32_t b = 0; b < nb; ++b) w |= (uint64_t)sp[b] << (56 - 8 * b);
+    const uint32_t mk = rest < RANK_WIN + 1 ? rest : RANK_WIN + 1;
+    uint8_t* k = keys + j * RANK_KEY;
+    for (int b = 0; b < 4; ++b) k[b] = (uint8_t)(g >> (24 - 8 * b));
+    for (int b = 0; b < 8; ++b) k[4 + b] = (uint8_t)(w >> (56 - 8 * b));
+    k[12] = (uint8_t)mk;
+    og |= g; ag &= g; ow |= w; aw &= w; om |= mk; am &= mk;
+  }
+  for (int d = 16; d; d >>= 1) {
+    og |= __shfl_xor_sync(0xFFFFFFFFu, og, d); ag &= __shfl_xor_sync(0xFFFFFFFFu, ag, d);
+    ow |= __shfl_xor_sync(0xFFFFFFFFu, ow, d); aw &= __shfl_xor_sync(0xFFFFFFFFu, aw, d);
+    om |= __shfl_xor_sync(0xFFFFFFFFu, om, d); am &= __shfl_xor_sync(0xFFFFFFFFu, am, d);
+  }
+  if ((threadIdx.x & 31) == 0) {
+    for (int b = 0; b < 4; ++b) rank_bits_put(bits, b, (og >> (24 - 8 * b)) & 0xFFu, (ag >> (24 - 8 * b)) & 0xFFu);
+    for (int b = 0; b < 8; ++b) rank_bits_put(bits, 4 + b, (uint32_t)(ow >> (56 - 8 * b)) & 0xFFu, (uint32_t)(aw >> (56 - 8 * b)) & 0xFFu);
+    rank_bits_put(bits, 12, om, am);
+  }
+}
+__device__ __forceinline__ bool rank_key_eq(const uint8_t* a, const uint8_t* b) {
+  for (int i = 0; i < RANK_KEY; ++i) if (a[i] != b[i]) return false;
+  return true;
+}
+// the sorted open rows back into their groups' positions; new group heads; flags[i] = open row | (first row of an open group) << 32
+__global__ void rank_refine_kernel(const uint8_t* __restrict__ keys, const uint32_t* __restrict__ idx, int64_t m, const uint32_t* __restrict__ opos,
+                                   const uint32_t* __restrict__ rowof, uint32_t* __restrict__ perm, uint32_t* __restrict__ head, uint64_t* __restrict__ flags) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < m; i += (int64_t)gridDim.x * blockDim.x) {
+    const uint32_t j = idx[i];
+    const uint8_t* kj = keys + (int64_t)j * RANK_KEY;
+    const uint32_t p = opos ? opos[i] : (uint32_t)i;
+    perm[p] = rowof ? rowof[j] : j;
+    const bool eq_prev = i > 0 && rank_key_eq(kj, keys + (int64_t)idx[i - 1] * RANK_KEY);
+    const bool eq_next = i + 1 < m && rank_key_eq(kj, keys + (int64_t)idx[i + 1] * RANK_KEY);
+    if (!eq_prev) head[p] = 1u;
+    const bool open = kj[12] == RANK_WIN + 1 && (eq_prev || eq_next);
+    flags[i] = (uint64_t)open | ((uint64_t)(open && !eq_prev) << 32);
+  }
+}
+// the open rows of the next round: their positions and dense open-group numbers (in position order); *count = how many
+__global__ void rank_compact_kernel(const uint64_t* __restrict__ flags, const uint64_t* __restrict__ before, int64_t m, const uint32_t* __restrict__ opos,
+                                    uint32_t* __restrict__ opos_out, uint32_t* __restrict__ grp_out, uint32_t* __restrict__ count) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < m; i += (int64_t)gridDim.x * blockDim.x) {
+    const uint64_t f = flags[i], b = before[i];      // low half: open rows before i; high half: open groups begun before i
+    if (f & 1u) {
+      opos_out[(uint32_t)b] = opos ? opos[i] : (uint32_t)i;
+      grp_out[(uint32_t)b] = (uint32_t)(b >> 32) + (uint32_t)(f >> 32) - 1u;
+    }
+    if (i == m - 1) *count = (uint32_t)b + (uint32_t)f;
+  }
+}
+__global__ void rank_assign_kernel(const uint32_t* __restrict__ perm, const uint32_t* __restrict__ head, const uint64_t* __restrict__ before, int64_t n,
+                                   uint32_t* __restrict__ rank) {
+  for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < n; p += (int64_t)gridDim.x * blockDim.x)
+    rank[perm[p]] = (uint32_t)(before[p] + head[p] - 1u);
+}
+
+cudaError_t string_ranks(const void* views, const uint8_t* validity, int64_t n, uint32_t* rank, const StringRankScratch& S, cudaStream_t s, int* launches,
+                         int* syncs) {
+  int nl = 0, ns = 0;
+  *launches = 0; *syncs = 0;
+  if (n == 0) return cudaSuccess;
+  auto grid = [](int64_t m) { return (int)std::min<int64_t>((m + 255) / 256, grid_cap(8)); };
+  const uint8_t* vw = static_cast<const uint8_t*>(views);
+  uint32_t* count = S.ctrl + 2 * RANK_KEY;
+  uint32_t hc[2 * RANK_KEY + 1];
+  cudaError_t e = cudaMemsetAsync(S.head, 0, (size_t)n * 4, s);
+  if (e != cudaSuccess) return e;
+  const uint32_t *opos = nullptr, *grp = nullptr;
+  int64_t m = n;                       // open rows of the round (an upper bound until the read-back)
+  for (uint32_t offset = 0, buf = 0;; offset += RANK_WIN, buf ^= 1) {
+    if ((e = cudaMemsetAsync(S.ctrl, 0, 2 * RANK_KEY * 4, s)) != cudaSuccess) return e;
+    rank_encode_kernel<<<grid(m), 256, 0, s>>>(vw, validity, n, offset ? count : nullptr, offset, opos, grp, S.perm, S.rowof, S.keys, S.ctrl);
+    ++nl;
+    // the one read-back of the round: how many rows are open, and which key bytes vary among them
+    if ((e = cudaMemcpyAsync(hc, S.ctrl, sizeof(hc), cudaMemcpyDeviceToHost, s)) != cudaSuccess) return e;
+    if ((e = cudaStreamSynchronize(s)) != cudaSuccess) return e;
+    ++ns;
+    if (offset) m = hc[2 * RANK_KEY];
+    if (m == 0) break;
+    int sl = 0;
+    if ((e = radix_sort_indices_host_bits(S.keys, RANK_KEY, m, S.radix, hc, s, &sl)) != cudaSuccess) return e;
+    rank_refine_kernel<<<grid(m), 256, 0, s>>>(S.keys, S.radix.idx_a, m, opos, opos ? S.rowof : nullptr, S.perm, S.head, S.flags);
+    if ((e = launch_exclusive_scan_u64(S.flags, m, S.before, S.scan_scratch, s)) != cudaSuccess) return e;
+    rank_compact_kernel<<<grid(m), 256, 0, s>>>(S.flags, S.before, m, opos, S.opos[buf], S.grp[buf], count);
+    nl += sl + 5;
+    opos = S.opos[buf]; grp = S.grp[buf];
+  }
+  if ((e = launch_exclusive_scan_u32(S.head, n, S.before, S.scan_scratch, s)) != cudaSuccess) return e;
+  rank_assign_kernel<<<grid(n), 256, 0, s>>>(S.perm, S.head, S.before, n, rank);
+  nl += 4;
+  *launches = nl; *syncs = ns;
+  return cudaGetLastError();
+}
+
+// ------------------------------------------------------------------------------------------------
+// TopK selection (SortExec with fetch = k, test_tpch.plan.yaml:27,79; ClickBench ORDER BY .. LIMIT 10): radix SELECT on
+// a 64-bit word per row instead of sorting all n rows.  One level = one streaming pass over 8 B/row: histogram of the next
+// 11 bits among the rows whose consumed prefix equals the threshold path.
+// ------------------------------------------------------------------------------------------------
+// The word is the leading 8 bytes of the order-preserving encoding, built from the key columns, except that a string key
+// contributes its own leading bytes (zero-padded, inverted when descending) and nothing comes after it.  It is monotone in the
+// requested order (a < b implies word(a) <= word(b)), which is all the selection needs; the candidates are then sorted exactly.
+__global__ void topk_word_kernel(const SortEncodeParams P, uint64_t* __restrict__ words) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < P.n; i += (int64_t)gridDim.x * blockDim.x) {
+    uint64_t w = 0;
+    int pos = 0;
+    auto put = [&](uint32_t b) { if (pos < 8) w |= (uint64_t)(b & 0xFFu) << (56 - 8 * pos); ++pos; };
+    for (int k = 0; k < P.n_keys && pos < 8; ++k) {
+      const SortKeyCol& c = P.cols[k];
+      const bool isnull = c.validity_bits && !((c.validity_bits[i >> 3] >> (i & 7)) & 1);
+      put(isnull ? (c.nulls_first ? 0x00 : 0xFF) : (c.nulls_first ? 0x01 : 0x00));
+      const uint32_t inv = c.asc ? 0x00 : 0xFF;
+      if (c.kind == SORT_VIEW) {
+        if (!isnull) {
+          const uint8_t* vp = c.data + i * 16;
+          const ulonglong2 v = *reinterpret_cast<const ulonglong2*>(vp);
+          const uint32_t len = (uint32_t)v.x;
+          const uint8_t* s = view_ptr(v, vp);
+          for (uint32_t b = 0; pos < 8; ++b) put((b < len ? s[b] : 0u) ^ inv);
+        }
+        break;
+      }
+      if (isnull) { pos += c.enc_bytes; continue; }
+      switch (c.kind) {
+        case SORT_INT:
+        case SORT_UINT: {
+          const uint8_t* p = c.data + i * c.width;
+          for (int b = 0; b < c.width && pos < 8; ++b) put(p[c.width - 1 - b] ^ inv ^ ((b == 0 && c.kind == SORT_INT) ? 0x80u : 0x00u));
+          break;
+        }
+        case SORT_F64: {
+          uint64_t v = *reinterpret_cast<const uint64_t*>(c.data + i * 8);
+          v = (v >> 63) ? ~v : (v | 0x8000000000000000ull);
+          for (int b = 0; b < 8 && pos < 8; ++b) put((uint32_t)(v >> (56 - 8 * b)) ^ inv);
+          break;
+        }
+        default:              // SORT_BOOL
+          put(((c.data[i >> 3] >> (i & 7)) & 1u) ^ inv);
+      }
+    }
+    words[i] = w;
+  }
+}
+cudaError_t launch_topk_words(const SortEncodeParams& P, uint64_t* words, cudaStream_t s) {
+  if (P.n == 0) return cudaSuccess;
+  topk_word_kernel<<<(int)std::min<int64_t>((P.n + 255) / 256, grid_cap(8)), 256, 0, s>>>(P, words);
+  return cudaGetLastError();
+}
+__global__ void topk_hist_kernel(const uint64_t* __restrict__ words, int64_t n, int used, uint64_t prefix, int digit_bits, uint32_t* __restrict__ hist) {
   __shared__ uint32_t sh[2048];
   for (int i = threadIdx.x; i < 2048; i += blockDim.x) sh[i] = 0;
   __syncthreads();
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    const uint64_t w = key_word_be(keys + i * key_bytes, key_bytes);
+    const uint64_t w = words[i];
     if (used == 0 || (w >> (64 - used)) == prefix) atomicAdd(&sh[(uint32_t)((w << used) >> (64 - digit_bits))], 1u);
   }
   __syncthreads();
   for (int i = threadIdx.x; i < 2048; i += blockDim.x) if (sh[i]) atomicAdd(&hist[i], sh[i]);
 }
-// rows whose leading `used` key bits are <= threshold (every row when used == 0): their indices, in any order
-__global__ void topk_compact_kernel(const uint8_t* __restrict__ keys, int key_bytes, int64_t n, int used, uint64_t threshold, int64_t* __restrict__ out, unsigned long long* counter) {
+// rows whose leading `used` word bits are <= threshold (every row when used == 0): their indices, in any order
+__global__ void topk_compact_kernel(const uint64_t* __restrict__ words, int64_t n, int used, uint64_t threshold, int64_t* __restrict__ out, unsigned long long* counter) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    const uint64_t w = key_word_be(keys + i * key_bytes, key_bytes);
+    const uint64_t w = words[i];
     const bool take = used == 0 || (w >> (64 - used)) <= threshold;
     const unsigned m = __ballot_sync(__activemask(), take);
     if (take) {
@@ -443,12 +620,12 @@ __global__ void topk_compact_kernel(const uint8_t* __restrict__ keys, int key_by
     }
   }
 }
-cudaError_t launch_topk_hist(const uint8_t* keys, int key_bytes, int64_t n, int used, uint64_t prefix, int digit_bits, uint32_t* hist, cudaStream_t s) {
-  topk_hist_kernel<<<(int)std::min<int64_t>((n + 255) / 256, grid_cap(8)), 256, 0, s>>>(keys, key_bytes, n, used, prefix, digit_bits, hist);
+cudaError_t launch_topk_hist(const uint64_t* words, int64_t n, int used, uint64_t prefix, int digit_bits, uint32_t* hist, cudaStream_t s) {
+  topk_hist_kernel<<<(int)std::min<int64_t>((n + 255) / 256, grid_cap(8)), 256, 0, s>>>(words, n, used, prefix, digit_bits, hist);
   return cudaGetLastError();
 }
-cudaError_t launch_topk_compact(const uint8_t* keys, int key_bytes, int64_t n, int used, uint64_t threshold, int64_t* out, unsigned long long* counter, cudaStream_t s) {
-  topk_compact_kernel<<<(int)std::min<int64_t>((n + 255) / 256, grid_cap(8)), 256, 0, s>>>(keys, key_bytes, n, used, threshold, out, counter);
+cudaError_t launch_topk_compact(const uint64_t* words, int64_t n, int used, uint64_t threshold, int64_t* out, unsigned long long* counter, cudaStream_t s) {
+  topk_compact_kernel<<<(int)std::min<int64_t>((n + 255) / 256, grid_cap(8)), 256, 0, s>>>(words, n, used, threshold, out, counter);
   return cudaGetLastError();
 }
 
@@ -487,39 +664,46 @@ cudaError_t launch_merge_rank(const uint8_t* keys, int key_bytes, const int64_t*
 }
 
 // sort-based grouping (aggregates whose group key does not fit the hash table's packed key).  Rows are ordered by a 64-bit hash of
-// their encoded key (8 radix digits instead of one per key byte: Q10's keys are ~250 bytes); `heads` marks the first row of every
-// run of equal ENCODED keys.  Two different keys with one hash would make equal keys non-adjacent: *collisions counts adjacent
-// rows with equal hash and different keys, and the caller falls back to ordering by the full key when it is not zero.
-__global__ void key_hash_kernel(const uint8_t* __restrict__ keys, int key_bytes, int64_t n, uint8_t* __restrict__ out8) {
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    const uint8_t* k = keys + i * key_bytes;
+// their key columns (8 radix digits whatever the key width; strings hashed whole, NULL a value of its own); `heads` marks the
+// first row of every run of equal keys (cmp_sort_key == 0 on every column).  Two different keys with one hash would make equal
+// keys non-adjacent: *collisions counts adjacent rows with equal hash and different keys, and the caller then orders by the key.
+__global__ void group_hash_kernel(const SortEncodeParams P, uint8_t* __restrict__ out8) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < P.n; i += (int64_t)gridDim.x * blockDim.x) {
     uint64_t h = 0x243F6A8885A308D3ull;
-    int j = 0;
-    for (; j + 8 <= key_bytes; j += 8) { uint64_t w = 0; for (int b = 0; b < 8; ++b) w |= (uint64_t)k[j + b] << (8 * b); h = mix64(h ^ w); }
-    if (j < key_bytes) { uint64_t w = 0; for (int b = 0; j + b < key_bytes; ++b) w |= (uint64_t)k[j + b] << (8 * b); h = mix64(h ^ w ^ ((uint64_t)key_bytes << 56)); }
+    for (int k = 0; k < P.n_keys; ++k) {
+      const SortKeyCol& c = P.cols[k];
+      if (c.validity_bits && !((c.validity_bits[i >> 3] >> (i & 7)) & 1)) { h = mix64(h ^ 0x9E3779B97F4A7C15ull); continue; }
+      if (c.kind == SORT_VIEW) { h = mix64(h ^ view_hash(*reinterpret_cast<const ulonglong2*>(c.data + i * 16))); continue; }
+      if (c.kind == SORT_BOOL) { h = mix64(h ^ ((c.data[i >> 3] >> (i & 7)) & 1u)); continue; }
+      const uint8_t* p = c.data + i * c.width;
+      for (int j = 0; j < c.width; j += 8) {
+        uint64_t w = 0;
+        for (int b = 0; b < 8 && j + b < c.width; ++b) w |= (uint64_t)p[j + b] << (8 * b);
+        h = mix64(h ^ w);
+      }
+    }
     for (int b = 0; b < 8; ++b) out8[i * 8 + b] = (uint8_t)(h >> (56 - 8 * b));      // big-endian: memcmp order == numeric order
   }
 }
-cudaError_t launch_key_hash(const uint8_t* keys, int key_bytes, int64_t n, uint8_t* out8, cudaStream_t s) {
-  if (n == 0) return cudaSuccess;
-  key_hash_kernel<<<(int)std::min<int64_t>((n + 255) / 256, grid_cap(8)), 256, 0, s>>>(keys, key_bytes, n, out8);
+cudaError_t launch_group_hash(const SortEncodeParams& P, uint8_t* out8, cudaStream_t s) {
+  if (P.n == 0) return cudaSuccess;
+  group_hash_kernel<<<(int)std::min<int64_t>((P.n + 255) / 256, grid_cap(8)), 256, 0, s>>>(P, out8);
   return cudaGetLastError();
 }
-__global__ void group_heads_kernel(const uint8_t* __restrict__ keys, int key_bytes, const uint32_t* __restrict__ idx, int64_t n, uint32_t* __restrict__ heads,
-                                   const uint8_t* __restrict__ hashes, unsigned long long* __restrict__ collisions) {
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+__global__ void group_heads_kernel(const SortEncodeParams P, const uint32_t* __restrict__ idx, uint32_t* __restrict__ heads,
+                                   const uint64_t* __restrict__ hashes, unsigned long long* __restrict__ collisions) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < P.n; i += (int64_t)gridDim.x * blockDim.x) {
     bool head = i == 0;
     if (i > 0) {
-      head = key_cmp(keys + (int64_t)idx[i] * key_bytes, keys + (int64_t)idx[i - 1] * key_bytes, key_bytes) != 0;
-      if (head && hashes && key_cmp(hashes + (int64_t)idx[i] * 8, hashes + (int64_t)idx[i - 1] * 8, 8) == 0) atomicAdd(collisions, 1ull);
+      for (int k = 0; k < P.n_keys && !head; ++k) head = cmp_sort_key(P.cols[k], idx[i], idx[i - 1]) != 0;
+      if (head && hashes && hashes[idx[i]] == hashes[idx[i - 1]]) atomicAdd(collisions, 1ull);
     }
     heads[i] = head ? 1u : 0u;
   }
 }
-cudaError_t launch_group_heads(const uint8_t* keys, int key_bytes, const uint32_t* idx, int64_t n, uint32_t* heads, const uint8_t* hashes,
-                               unsigned long long* collisions, cudaStream_t s) {
-  if (n == 0) return cudaSuccess;
-  group_heads_kernel<<<(int)std::min<int64_t>((n + 255) / 256, grid_cap(8)), 256, 0, s>>>(keys, key_bytes, idx, n, heads, hashes, collisions);
+cudaError_t launch_group_heads(const SortEncodeParams& P, const uint32_t* idx, uint32_t* heads, const uint8_t* hashes, unsigned long long* collisions, cudaStream_t s) {
+  if (P.n == 0) return cudaSuccess;
+  group_heads_kernel<<<(int)std::min<int64_t>((P.n + 255) / 256, grid_cap(8)), 256, 0, s>>>(P, idx, heads, reinterpret_cast<const uint64_t*>(hashes), collisions);
   return cudaGetLastError();
 }
 // group number of every input row (dense, in key order) and one representative input row per group

@@ -42,8 +42,7 @@ struct SortKeyCol {
   int32_t asc, nulls_first;
   int32_t out_off;                // offset of this key inside the encoded row
   int32_t enc_bytes;              // value bytes after the null byte
-  int32_t str_len;                // SORT_VIEW: padded string bytes (max length in the column)
-  int32_t pad;
+  const uint32_t* rank;           // SORT_VIEW, encoded sort: the dense rank of every row's string (string_ranks)
 };
 struct SortEncodeParams {
   int64_t n;
@@ -59,6 +58,15 @@ struct RadixScratch {
   uint64_t* offs;                 // [256 * ceil(n / 2048)]
   uint64_t* scan_scratch;         // [1026]
 };
+struct StringRankScratch {
+  RadixScratch radix;             // for n rows
+  uint8_t* keys;                  // [13 * n]
+  uint32_t *perm, *head, *rowof;  // [n]
+  uint32_t *opos[2], *grp[2];     // [n]
+  uint64_t *flags, *before;       // [n]
+  uint64_t* scan_scratch;         // [1026]
+  uint32_t* ctrl;                 // [27]
+};
 
 cudaError_t launch_join_multi(const JoinMultiParams& P, cudaStream_t s);
 cudaError_t launch_gather_bits(const uint8_t* bits, uint8_t* out, const int64_t* idx, int64_t n, int dflt, cudaStream_t s);
@@ -68,12 +76,19 @@ cudaError_t launch_sort_encode(const SortEncodeParams& P, cudaStream_t s);
 constexpr int SMALL_SORT_ROWS = 1024;
 cudaError_t launch_small_sort_cols(const SortEncodeParams& P, uint32_t* idx_out, cudaStream_t s);
 cudaError_t radix_sort_indices(const uint8_t* keys, int key_bytes, int64_t n, const RadixScratch& S, const uint32_t* bits, cudaStream_t s, int* launches);
-cudaError_t launch_topk_hist(const uint8_t* keys, int key_bytes, int64_t n, int used, uint64_t prefix, int digit_bits, uint32_t* hist /* [2048], zeroed */, cudaStream_t s);
-cudaError_t launch_topk_compact(const uint8_t* keys, int key_bytes, int64_t n, int used, uint64_t threshold, int64_t* out, unsigned long long* counter, cudaStream_t s);
+cudaError_t radix_sort_indices_host_bits(const uint8_t* keys, int key_bytes, int64_t n, const RadixScratch& S, const uint32_t* host_bits, cudaStream_t s, int* launches);
+// rank[row] = dense rank of the row's string among the n views (memcmp order, a prefix before its extensions; null rows rank as
+// ""), for n < 2^32.  Synchronises the stream once per 8-byte window that some group of equal prefixes still spans (*syncs).
+cudaError_t string_ranks(const void* views, const uint8_t* validity, int64_t n, uint32_t* rank, const StringRankScratch& S, cudaStream_t s, int* launches,
+                         int* syncs);
+cudaError_t launch_topk_words(const SortEncodeParams& P, uint64_t* words, cudaStream_t s);
+cudaError_t launch_topk_hist(const uint64_t* words, int64_t n, int used, uint64_t prefix, int digit_bits, uint32_t* hist /* [2048], zeroed */, cudaStream_t s);
+cudaError_t launch_topk_compact(const uint64_t* words, int64_t n, int used, uint64_t threshold, int64_t* out, unsigned long long* counter, cudaStream_t s);
 cudaError_t launch_merge_rank(const uint8_t* keys, int key_bytes, const int64_t* run_off, int n_runs, int64_t n, int64_t* perm, cudaStream_t s);
-cudaError_t launch_key_hash(const uint8_t* keys, int key_bytes, int64_t n, uint8_t* out8, cudaStream_t s);
-cudaError_t launch_group_heads(const uint8_t* keys, int key_bytes, const uint32_t* idx, int64_t n, uint32_t* heads, const uint8_t* hashes,
-                               unsigned long long* collisions, cudaStream_t s);
+cudaError_t launch_group_hash(const SortEncodeParams& P, uint8_t* out8, cudaStream_t s);
+// heads[i] = 1 where row idx[i] differs from row idx[i - 1] in some key column of P (P.n rows); with `hashes`, *collisions counts
+// heads whose 8-byte hash equals the previous row's
+cudaError_t launch_group_heads(const SortEncodeParams& P, const uint32_t* idx, uint32_t* heads, const uint8_t* hashes, unsigned long long* collisions, cudaStream_t s);
 cudaError_t launch_assign_groups(const uint32_t* idx, const uint32_t* heads, const uint64_t* before, int64_t n, int64_t* gid_of_row, int64_t* rep, cudaStream_t s);
 cudaError_t launch_iota(int64_t* out, int64_t n, cudaStream_t s);
 cudaError_t launch_iota_stride(int64_t* out, int64_t first, int64_t stride, int64_t n, cudaStream_t s);
