@@ -36,11 +36,22 @@
  *   {"op":"filter","predicate":E,"projection":[i,...]|null}
  *   {"op":"projection","exprs":[{"expr":E,"name":"..."},...]}
  *   {"op":"aggregate","mode":"partial|final|final_partitioned|single",
- *    "group_by":[{"expr":E,"name":".."}],"aggs":[{"fn":"sum|avg|count|min|max","args":[E],
+ *    "group_by":[{"expr":E,"name":".."}],"aggs":[{"fn":"sum|avg|count|min|max|stddev|stddev_pop|var|var_pop","args":[E],
  *    "name":"..","input_type":"T","distinct":false|true}]}
  *                                          ("distinct": true -- count / sum / avg(DISTINCT E) -- in mode single only, over one
  *                                           argument that is not Float32 / Float64 / Boolean, at most 4 distinct arguments per
  *                                           aggregate; for min / max the flag is a no-op)
+ *                                          (stddev / var: the sample forms, stddev_pop / var_pop: the population forms, under
+ *                                           DataFusion's physical names; aliases such as variance or stddev_samp are refused.
+ *                                           The argument is any integer, Decimal128, Float32 or Float64, converted to Float64;
+ *                                           the result is Float64, NULL below 2 (sample) or 1 (population) non-null values.
+ *                                           Partial state: name[count] UInt64, name[mean] Float64, name[m2] Float64 (sum of
+ *                                           squared deviations; 0, 0.0, 0.0 for a group without values).  Sums are kept in
+ *                                           double-double, so results stay within about 1e-10 relative even where |mean| / stddev
+ *                                           is 1e8; equal values give exactly 0.0.  A group holding NaN or +-inf gives NaN, a
+ *                                           single one included (DataFusion's ungrouped accumulator reports 0.0 for var_pop of
+ *                                           one non-finite value), and so does a value whose square leaves Float64 (|x| above
+ *                                           about 1.3e154); the partial mean and m2 of such a group are NaN.)
  *   {"op":"hash_join","join_type":"inner|left|right|left_semi|left_anti|right_semi|right_anti","on":[[l,r],...],
  *    "filter":E|null,"projection":[...]|null}   (input 0 = build = LEFT child, input 1 = probe; residual filters with
  *                                           inner, right_semi, left_semi and left_anti)

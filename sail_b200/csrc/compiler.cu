@@ -365,12 +365,14 @@ void PipelineCompiler::finish_aggregate(CompiledPipeline& out, const StageSpec& 
     SG_CHECK(A.n_accs < MAX_ACCS, SAILGPU_ERR_UNSUPPORTED, "more than " + std::to_string(MAX_ACCS) + " distinct accumulators");
     AccDesc d{}; d.op = (uint8_t)op; d.vkind = (uint8_t)vkind; d.stride = (uint8_t)stride;
     d.value_slot = vslot >= 0 ? (uint32_t)vslot : NO_SLOT; d.valid_slot = valid >= 0 ? (uint32_t)valid : NO_SLOT;
-    d.track_seen = (op != ACC_COUNT && (valid >= 0 || A.n_keys == 0)) ? 1 : 0;
-    // a 128-bit min / max is updated by a 16-byte compare-and-swap, which needs a 16-byte aligned address: it starts on an
-    // even word of its entry (and entries are an even number of words long, below)
-    if ((op == ACC_MIN_I128 || op == ACC_MAX_I128) && ((2 + A.key_words + words) & 1)) ++words;
+    d.n_slot = d.mean_slot = NO_SLOT;
+    // a variance accumulator's nulls come from its count
+    d.track_seen = (op != ACC_COUNT && !acc_is_dd(op) && (valid >= 0 || A.n_keys == 0)) ? 1 : 0;
+    // a 128-bit min / max and a double-double sum are updated by a 16-byte compare-and-swap, which needs a 16-byte aligned
+    // address: they start on an even word of their entry (and entries are an even number of words long, below)
+    if ((op == ACC_MIN_I128 || op == ACC_MAX_I128 || acc_is_dd(op)) && ((2 + A.key_words + words) & 1)) ++words;
     d.word = (uint16_t)words;
-    words += (op == ACC_SUM_I128 || op == ACC_MIN_I128 || op == ACC_MAX_I128) ? 2 : 1;
+    words += (op == ACC_SUM_I128 || op == ACC_MIN_I128 || op == ACC_MAX_I128 || acc_is_dd(op)) ? 2 : 1;
     A.accs[A.n_accs] = d;
     dedup[key] = A.n_accs;
     return A.n_accs++;
@@ -421,12 +423,50 @@ void PipelineCompiler::finish_aggregate(CompiledPipeline& out, const StageSpec& 
     }
   };
 
+  // variance family: count, a double-double sum and a double-double sum of squares of the argument as Float64 (the count is the
+  // argument's count|, shared with count / avg over it).  Merging, a state row's count is summed and its (count, mean, m2) feed
+  // both sums: the sum reads the mean as its value, the sum of squares m2, and both the count and the mean (AccDesc::n_slot /
+  // mean_slot).
+  struct Moments { int jc, js, jq; };
+  std::map<std::string, Val> as_f64;   // the argument as Float64, once per argument
+  auto moments = [&](const Val& x0, const ExprPtr& x_expr, const DataType& t, const std::string& id, bool merge_rows) -> Moments {
+    Moments m{};
+    if (!merge_rows) {
+      auto it = as_f64.find(id);
+      if (it == as_f64.end()) {
+        Val f;
+        // a UInt64 lives in an I64 slot, which the cast would convert as signed
+        if (t.id == TypeId::UInt64) { f = emit1(OP_CVT, K_F64, K_F64, x0, SRC_U64); f.vslot = x0.vslot; }
+        else f = compile(make_cast(x_expr, T(TypeId::Float64)));
+        it = as_f64.emplace(id, ensure_slot(f)).first;
+      }
+      const Val f = it->second;
+      if (x0.vslot >= 0) { Val only_valid = x0; m.jc = add_acc(ACC_COUNT, &only_valid); } else m.jc = add_acc(ACC_COUNT, nullptr);
+      ident("count|" + id, m.jc);
+      m.js = ident("ddsum|" + id, add_acc(ACC_DD_SUM, &f));
+      m.jq = ident("ddsq|" + id, add_acc(ACC_DD_SQ, &f));
+      return m;
+    }
+    Val c = compile(bindings_.at(state_col_ + 0)), mean = compile(bindings_.at(state_col_ + 1)), m2 = compile(bindings_.at(state_col_ + 2));
+    Val w = convert(c, K_I64); w.vslot = c.vslot;
+    m.jc = ident("count|" + id, add_acc(ACC_SUM_I64, &w)); A.accs[m.jc].track_seen = 0;
+    Val n = ensure_slot(convert(c, K_F64));
+    Val mf = ensure_slot(convert(mean, K_F64)), qf = ensure_slot(convert(m2, K_F64));
+    SG_CHECK(n.stride == 8 && mf.stride == 8, SAILGPU_ERR_INVALID, "variance state columns must be Float64");
+    mf.vslot = c.vslot; qf.vslot = c.vslot;
+    m.js = ident("ddsum|" + id, add_acc(ACC_DD_SUM, &mf));
+    m.jq = ident("ddsq|" + id, add_acc(ACC_DD_SQ, &qf));
+    for (int j : {m.js, m.jq}) { A.accs[j].n_slot = (uint32_t)n.slot; A.accs[j].mean_slot = (uint32_t)mf.slot; }
+    return m;
+  };
+
   // output columns: group keys first
   for (int i = 0; i < A.n_keys; ++i) {
     AggOutSpec o{}; o.kind = 0; o.a = i; o.b = key_first_word[(size_t)i]; o.type = key_types[(size_t)i]; o.nullable = A.keys[i].valid_slot != NO_SLOT;
     out.agg_outs.push_back(o);
   }
-  size_t state_col = st.group_exprs.size();   // merging: cursor into the input state columns (current bindings)
+  size_t& state_col = state_col_;   // merging: cursor into the input state columns (current bindings)
+  state_col = st.group_exprs.size();
   for (auto& a : st.aggs) {
     DataType in_t = a.input_type;
     Val arg; bool has_arg = false;
@@ -486,11 +526,29 @@ void PipelineCompiler::finish_aggregate(CompiledPipeline& out, const StageSpec& 
       } else {
         push_out(2, js, jc, at.final_type, true);
       }
+    } else if (is_variance_fn(a.fn)) {
+      const Moments mo = moments(arg, merging ? nullptr : substitute(a.arg), in_t, merging ? "state" + std::to_string(state_col) : aid, merging);
+      if (partial) {
+        push_out(1, mo.jc, 0, T(TypeId::UInt64), false);
+        push_out(3, mo.js, mo.jc, T(TypeId::Float64), false);
+        AggOutSpec o{}; o.kind = 4; o.a = mo.jq; o.b = mo.jc; o.c = mo.js; o.type = T(TypeId::Float64); o.nullable = false; o.in_type = in_t;
+        out.agg_outs.push_back(o);
+      } else {
+        AggOutSpec o{}; o.kind = 5; o.a = mo.jq; o.b = mo.jc; o.c = mo.js; o.type = T(TypeId::Float64); o.nullable = true; o.in_type = in_t;
+        o.var = variance_flags(a.fn);
+        out.agg_outs.push_back(o);
+      }
     } else fail(SAILGPU_ERR_UNSUPPORTED, "aggregate function '" + a.fn + "'");
     state_col += at.state.size();
   }
+  {   // the extraction kernel takes at most MAX_KEYS + 2 * MAX_ACCS columns, in the operator's output and in the state rows
+    size_t n_state = st.group_exprs.size();
+    for (auto& a : st.aggs) n_state += agg_types(a.fn, a.fn == "count" ? T(TypeId::Int64) : a.input_type).state.size();
+    SG_CHECK(std::max(out.agg_outs.size(), n_state) <= (size_t)(MAX_KEYS + 2 * MAX_ACCS), SAILGPU_ERR_UNSUPPORTED,
+             "aggregate with more than " + std::to_string(MAX_KEYS + 2 * MAX_ACCS) + " output or state columns");
+  }
   bool cas128 = false;
-  for (int j = 0; j < A.n_accs; ++j) cas128 |= A.accs[j].op == ACC_MIN_I128 || A.accs[j].op == ACC_MAX_I128;
+  for (int j = 0; j < A.n_accs; ++j) cas128 |= A.accs[j].op == ACC_MIN_I128 || A.accs[j].op == ACC_MAX_I128 || acc_is_dd(A.accs[j].op);
   if (cas128 && ((2 + A.key_words + words) & 1)) ++words;
   A.acc_words = words;
   A.entry_words = (uint32_t)(2 + A.key_words + A.acc_words);
@@ -631,7 +689,10 @@ void PipelineCompiler::finalize(CompiledPipeline& out, Ctx* ctx, int hot_wanted)
     AggParams& AA = out.agg;
     for (int i = 0; i < AA.n_keys; ++i) { AA.keys[i].slot = off(AA.keys[i].slot); AA.keys[i].valid_slot = off(AA.keys[i].valid_slot); }
     for (int w = AA.has_null_word; w < AA.key_words; ++w) { AA.kwords[w].slot = off(AA.kwords[w].slot); AA.kwords[w].valid_slot = off(AA.kwords[w].valid_slot); }
-    for (int j = 0; j < AA.n_accs; ++j) { AA.accs[j].value_slot = off(AA.accs[j].value_slot); AA.accs[j].valid_slot = off(AA.accs[j].valid_slot); }
+    for (int j = 0; j < AA.n_accs; ++j) {
+      AA.accs[j].value_slot = off(AA.accs[j].value_slot); AA.accs[j].valid_slot = off(AA.accs[j].valid_slot);
+      AA.accs[j].n_slot = off(AA.accs[j].n_slot); AA.accs[j].mean_slot = off(AA.accs[j].mean_slot);
+    }
     for (AggParams& D : out.distinct)
       for (int i = 0; i < D.n_keys; ++i) { D.keys[i].slot = off(D.keys[i].slot); D.keys[i].valid_slot = off(D.keys[i].valid_slot); }
     for (int j = 0; j < AA.n_accs && j < REG_ACCS; ++j) {

@@ -44,7 +44,9 @@ struct StageSpec {
 };
 
 // what one aggregate output column is made of
-struct AggOutSpec { int kind; int a, b; DataType type; bool nullable; DataType in_type; };
+// kind: 0 group key a (first word b), 1 accumulator a, 2 avg (sum a / count b); the variance family over a count b, a
+// double-double sum and sum of squares: 3 the mean (sum a), 4 m2 (sum of squares a, sum c), 5 var / stddev (as 4; var: VAR_*)
+struct AggOutSpec { int kind; int a, b; DataType type; bool nullable; DataType in_type; int c = 0; int var = 0; };
 
 // The pipeline before slot ids were rewritten to arena offsets: input of the kernel specialiser (jit.cu), which turns
 // slots into registers and needs to know who reads what.
@@ -218,6 +220,7 @@ class PipelineCompiler {
   std::vector<std::string> literals_;
   std::vector<std::pair<int, int>> literal_fixups_;
   std::vector<int> probe_slot_refs_;
+  size_t state_col_ = 0;               // finish_aggregate, merging: the first input column of the current aggregate's state
   bool small_acc_[MAX_ACCS] = {};      // accumulator input is statically below 2^55 (decimal precision <= 16)
   std::vector<OutputCol> outs_;
   std::vector<DataType> out_types_;

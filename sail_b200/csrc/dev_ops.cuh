@@ -180,6 +180,55 @@ __device__ __forceinline__ void atomic_minmax_f64(uint64_t* w, double v, bool is
   }
 }
 
+// ---- double-double arithmetic (the variance accumulators) ----------------------------------------------------------
+// A value is hi + lo with |lo| <= ulp(hi) / 2: about 106 significant bits.  The adds below are the accurate ("IEEE") variant,
+// whose relative error stays near 2^-104 whatever the signs, so sums of many terms keep about 100 bits.
+__device__ __forceinline__ void dd_two_sum(double a, double b, double& s, double& e) {
+  s = a + b; const double bb = s - a; e = (a - (s - bb)) + (b - bb);
+}
+__device__ __forceinline__ void dd_fast_two_sum(double a, double b, double& s, double& e) { s = a + b; e = b - (s - a); }
+__device__ __forceinline__ void dd_add(double& ah, double& al, double bh, double bl) {
+  double s, e, t, f;
+  dd_two_sum(ah, bh, s, e);
+  dd_two_sum(al, bl, t, f);
+  e += t;
+  dd_fast_two_sum(s, e, s, e);
+  e += f;
+  dd_fast_two_sum(s, e, ah, al);
+}
+// n * (h + l) for an integral n below 2^53
+__device__ __forceinline__ void dd_mul_d(double h, double l, double n, double& rh, double& rl) {
+  const double p = h * n;
+  const double e = fma(h, n, -p) + l * n;
+  dd_fast_two_sum(p, e, rh, rl);
+}
+// one row's (or one state row's) term of a variance accumulator as a double-double: x, x^2 exactly, or, merging a state row of
+// count n, mean and m2 (x = mean or m2), n * mean and m2 + n * mean^2
+__device__ __forceinline__ void dd_term(int op, double x, double n, double mean, bool merging, double& h, double& l) {
+  if (!merging) {
+    if (op == ACC_DD_SUM) { h = x; l = 0.0; }
+    else { h = x * x; l = fma(x, x, -h); }
+    return;
+  }
+  if (op == ACC_DD_SUM) { h = n * mean; l = fma(n, mean, -h); return; }
+  const double sq = mean * mean, sq_lo = fma(mean, mean, -sq);
+  dd_mul_d(sq, sq_lo, n, h, l);
+  dd_add(h, l, x, 0.0);
+}
+// 16-byte compare-and-swap loop: the table entry's double-double += (h, l)
+__device__ __forceinline__ void atomic_add_dd(uint64_t* w, double h, double l) {
+  if (h == 0.0 && l == 0.0) return;
+  u128 cur = ((u128)w[1] << 64) | w[0];
+  for (;;) {
+    double ch = __longlong_as_double((long long)(uint64_t)cur), cl = __longlong_as_double((long long)(uint64_t)(cur >> 64));
+    dd_add(ch, cl, h, l);
+    const u128 want = ((u128)(uint64_t)__double_as_longlong(cl) << 64) | (uint64_t)__double_as_longlong(ch);
+    const u128 prev = atomic_cas_128(w, cur, want);
+    if (prev == cur) return;
+    cur = prev;
+  }
+}
+
 // identity of accumulator word `word_in_acc` (0 or 1)
 __host__ __device__ inline uint64_t acc_identity(int op, int word_in_acc) {
   switch (op) {
@@ -193,7 +242,7 @@ __host__ __device__ inline uint64_t acc_identity(int op, int word_in_acc) {
   }
 }
 __host__ __device__ inline int acc_words_of(int op) {
-  return (op == ACC_SUM_I128 || op == ACC_MIN_I128 || op == ACC_MAX_I128) ? 2 : 1;
+  return (op == ACC_SUM_I128 || op == ACC_MIN_I128 || op == ACC_MAX_I128 || acc_is_dd(op)) ? 2 : 1;
 }
 
 // combine value into a (private or CTA-total) accumulator held in plain memory words
@@ -208,6 +257,12 @@ __device__ __forceinline__ void acc_combine_words(int op, uint64_t& w0, uint64_t
     case ACC_MAX_I128: { i128 a = (i128)(((u128)w1 << 64) | w0), b = (i128)(((u128)v1 << 64) | v0); if (b > a) { w0 = v0; w1 = v1; } break; }
     case ACC_MIN_F64: if (__longlong_as_double((long long)v0) < __longlong_as_double((long long)w0)) w0 = v0; break;
     case ACC_MAX_F64: if (__longlong_as_double((long long)v0) > __longlong_as_double((long long)w0)) w0 = v0; break;
+    case ACC_DD_SUM: case ACC_DD_SQ: {
+      double h = __longlong_as_double((long long)w0), l = __longlong_as_double((long long)w1);
+      dd_add(h, l, __longlong_as_double((long long)v0), __longlong_as_double((long long)v1));
+      w0 = (uint64_t)__double_as_longlong(h); w1 = (uint64_t)__double_as_longlong(l);
+      break;
+    }
     default: break;
   }
 }

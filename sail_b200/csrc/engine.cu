@@ -111,6 +111,11 @@ StageSpec parse_stage(const Json& j, const Schema& in, Schema* out) {
       state_col += at.state.size();
       if (st.mode == "partial") {
         if (ag.fn == "avg") { out->push_back({ag.name + "[count]", at.state[0], false}); out->push_back({ag.name + "[sum]", at.state[1], true}); }
+        else if (is_variance_fn(ag.fn)) {
+          out->push_back({ag.name + "[count]", at.state[0], false});
+          out->push_back({ag.name + "[mean]", at.state[1], false});
+          out->push_back({ag.name + "[m2]", at.state[2], false});
+        }
         else out->push_back({ag.name + "[" + ag.fn + "]", at.state[0], ag.fn != "count"});
       } else {
         out->push_back({ag.name, at.final_type, ag.fn != "count"});
@@ -707,12 +712,12 @@ struct PipelineOp : Op {
     for (int i = 0; i < X.n_cols; ++i) {
       const AggOutSpec& s = outs[(size_t)i];
       AggOutCol& o = X.cols[i];
-      o.kind = s.kind; o.a = s.a; o.b = s.b; o.nullable = s.nullable ? 1 : 0;
+      o.kind = s.kind; o.a = s.a; o.b = s.b; o.c = s.c; o.var = s.var; o.nullable = s.nullable ? 1 : 0;
       o.width = s.type.is_string() ? 16 : s.type.arrow_width();
       SG_CHECK(s.type.id != TypeId::Bool, SAILGPU_ERR_UNSUPPORTED, "boolean group keys are not supported yet");
       if (s.kind == 0) { o.key_word = s.b; o.src_words = A0.keys[s.a].width == 16 ? 2 : 1; }
       else if (s.kind == 1) { const int op = A0.accs[s.a].op; o.src_words = (op == ACC_SUM_I128 || op == ACC_MIN_I128 || op == ACC_MAX_I128) ? 2 : 1; }
-      else {
+      else if (s.kind == 2) {
         o.is_float = s.type.is_float() ? 1 : 0;
         if (!o.is_float) { i128 mul = pow10_i128(s.type.scale - s.in_type.scale); o.scale_mul_lo = (uint64_t)(u128)mul; o.scale_mul_hi = (uint64_t)((u128)mul >> 64); }
       }
@@ -774,10 +779,18 @@ struct PipelineOp : Op {
   // State rows as a partial aggregate emits them: keys, then each aggregate's state columns.  Every mode's table holds the
   // accumulators of those states (compiler.cu finish_aggregate: single and partial compile the same accumulators, the final
   // modes merge state columns into accumulators of the same kinds, avg as a count and a sum, Decimal128 sums in 128 bits);
-  // only the outputs differ, where avg is sum / count.
+  // only the outputs differ, where avg is sum / count and the variance family's count, mean and m2 become one value.
   static std::vector<AggOutSpec> state_outs(const CompiledPipeline& cp) {
     std::vector<AggOutSpec> outs;
     for (const AggOutSpec& s : cp.agg_outs) {
+      if (s.kind == 5) {
+        AggOutSpec c = s, mean = s, m2 = s;
+        c.kind = 1; c.a = s.b; c.b = 0; c.type = T(TypeId::UInt64); c.nullable = false;
+        mean.kind = 3; mean.a = s.c; mean.nullable = false;
+        m2.kind = 4; m2.nullable = false;
+        outs.push_back(c); outs.push_back(mean); outs.push_back(m2);
+        continue;
+      }
       if (s.kind != 2) { outs.push_back(s); continue; }
       AggOutSpec c = s, v = s;
       c.kind = 1; c.a = s.b; c.b = 0; c.type = T(TypeId::UInt64); c.nullable = false;

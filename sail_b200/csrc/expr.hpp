@@ -306,6 +306,11 @@ inline ExprPtr parse_expr(const Json& j, const Schema& in) {
 }
 
 // ---- aggregate typing (DataFusion UDAFs; SURVEY.md Appendix A) ------------------------------------
+// The variance family under the names DataFusion's physical plan gives its UDAFs: stddev and var are the sample forms.
+inline bool is_variance_fn(const std::string& fn) { return fn == "stddev" || fn == "stddev_pop" || fn == "var" || fn == "var_pop"; }
+inline int variance_flags(const std::string& fn) {
+  return (fn == "stddev_pop" || fn == "var_pop" ? VAR_POP : 0) | (fn == "stddev" || fn == "stddev_pop" ? VAR_SQRT : 0);
+}
 struct AggTypes { std::vector<DataType> state; DataType final_type; };
 inline AggTypes agg_types(const std::string& fn, const DataType& in) {
   AggTypes t;
@@ -325,6 +330,13 @@ inline AggTypes agg_types(const std::string& fn, const DataType& in) {
       t.state = {T(TypeId::UInt64), T(TypeId::Float64)};
       t.final_type = T(TypeId::Float64);
     }
+    return t;
+  }
+  if (is_variance_fn(fn)) {
+    // DataFusion coerces the argument to Float64; its state is the count, mean and sum of squared deviations
+    SG_CHECK(in.is_int() || in.is_decimal() || in.is_float(), SAILGPU_ERR_INVALID, fn + " over " + in.str());
+    t.state = {T(TypeId::UInt64), T(TypeId::Float64), T(TypeId::Float64)};
+    t.final_type = T(TypeId::Float64);
     return t;
   }
   fail(SAILGPU_ERR_UNSUPPORTED, "aggregate function '" + fn + "'");

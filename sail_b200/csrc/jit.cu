@@ -142,6 +142,10 @@ struct Emitter {
       case OP_CVT: {
         static const char* src_t[] = {"int8_t", "int16_t", "uint8_t", "uint16_t", "uint32_t", "float", "int32_t", "int64_t", "double", "i128", "bool"};
         static const int src_k[] = {-1, -1, -1, -1, -1, -1, K_I32, K_I64, K_F64, K_I128, K_B};
+        if (I.aux == SRC_U64) {   // UInt64 -> Float64, rounded once
+          if (kind != K_F64) throw Unsupported{"CVT from UInt64 to an integer"};
+          def(I.dst, kind, "(double)(uint64_t)" + operand(I.a, K_I64, I.sa)); break;
+        }
         if (I.aux > SRC_B) throw Unsupported{"CVT source"};
         std::string x;
         if (is_input((int)I.a)) x = (src_k[I.aux] >= 0 && src_k[I.aux] != K_B) ? operand(I.a, src_k[I.aux], I.sa) : raw_load(I.a, src_t[I.aux], I.sa);
@@ -310,6 +314,13 @@ struct Emitter {
         else if (d.vkind == K_B) o << " v.i = " << f << " ? 1 : 0;";
         else if (d.vkind == K_V16) throw Unsupported{"string accumulator"};
         else o << " v.i = (i128)" << f << ";";
+      }
+      if (acc_is_dd(d.op)) {   // the double-double term (pipeline.cu set_dd_value): high part in f, low part in i
+        if (d.vkind != K_F64) throw Unsupported{"variance accumulator over a non-Float64 slot"};
+        const bool merging = d.n_slot != NO_SLOT;
+        const std::string n = merging ? "o." + field(d.n_slot, K_F64, 8) : "0.0", mean = merging ? "o." + field(d.mean_slot, K_F64, 8) : "0.0";
+        o << " { double h, l; dd_term(" << (int)d.op << ", v.f, " << n << ", " << mean << ", " << (merging ? "true" : "false")
+          << ", h, l); v.f = h; v.i = (i128)(uint64_t)__double_as_longlong(l); }";
       }
       o << " }\n";
     }

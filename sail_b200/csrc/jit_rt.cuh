@@ -188,6 +188,7 @@ __device__ __forceinline__ void jit_acc_global(uint64_t* e, const AccVal& v) {
   else if constexpr (op == ACC_MAX_I128) atomic_minmax_i128(w, v.i, false);
   else if constexpr (op == ACC_MIN_F64) atomic_minmax_f64(w, v.f, true);
   else if constexpr (op == ACC_MAX_F64) atomic_minmax_f64(w, v.f, false);
+  else if constexpr (acc_is_dd(op)) atomic_add_dd(w, v.f, __longlong_as_double((long long)i128_lo(v.i)));
   if constexpr (G::acc_seen(J) != 0) {
     const unsigned long long bit = 1ull << J;
     if (!(*reinterpret_cast<volatile unsigned long long*>(e + 1) & bit)) atomicOr(reinterpret_cast<unsigned long long*>(e + 1), bit);
@@ -299,6 +300,7 @@ __device__ __forceinline__ void jit_acc_prepare(AccVal& v) {
   if constexpr (op == ACC_COUNT) { v.i = v.valid ? 1 : 0; }
   else if constexpr (op == ACC_SUM_I64 || op == ACC_SUM_I128) { if (!v.valid) v.i = 0; }
   else if constexpr (op == ACC_SUM_F64) { if (!v.valid) v.f = 0.0; }
+  else if constexpr (acc_is_dd(op)) { if (!v.valid) { v.f = 0.0; v.i = 0; } }
 }
 template <class G, int J>
 __device__ __forceinline__ void jit_acc_merge(AccVal& a, const AccVal& b) {
@@ -309,6 +311,11 @@ __device__ __forceinline__ void jit_acc_merge(AccVal& a, const AccVal& b) {
   else if constexpr (op == ACC_MAX_I32 || op == ACC_MAX_I64 || op == ACC_MAX_I128) { if (b.valid && (!a.valid || b.i > a.i)) { a.i = b.i; a.valid = true; } }
   else if constexpr (op == ACC_MIN_F64) { if (b.valid && (!a.valid || b.f < a.f)) { a.f = b.f; a.valid = true; } }
   else if constexpr (op == ACC_MAX_F64) { if (b.valid && (!a.valid || b.f > a.f)) { a.f = b.f; a.valid = true; } }
+  else if constexpr (acc_is_dd(op)) {
+    double h = a.f, l = __longlong_as_double((long long)i128_lo(a.i));
+    dd_add(h, l, b.f, __longlong_as_double((long long)i128_lo(b.i)));
+    a.f = h; a.i = (i128)(uint64_t)__double_as_longlong(l); a.valid = a.valid || b.valid;
+  }
 }
 template <class G, int J>
 __device__ __forceinline__ void jit_acc_global_n(uint64_t* e, const AccVal& v) {
@@ -587,9 +594,9 @@ __device__ __forceinline__ void jit_agg_dict_tile(const KernelArgs& K, const typ
 #pragma unroll
           for (int k = 0; k < G::RPT; ++k) {
             if (ok[k] && gid[k] == g) {
-              constexpr bool isf = op == ACC_MIN_F64 || op == ACC_MAX_F64;
+              constexpr bool isf = op == ACC_MIN_F64 || op == ACC_MAX_F64 || acc_is_dd(op);
               const uint64_t v0 = isf ? (uint64_t)__double_as_longlong(av[k].f) : i128_lo(av[k].i);
-              const uint64_t v1 = isf ? 0 : i128_hi(av[k].i);
+              const uint64_t v1 = acc_is_dd(op) ? i128_lo(av[k].i) : isf ? 0 : i128_hi(av[k].i);
               acc_combine_words(op, w0, w1, v0, v1);
             }
           }
@@ -657,6 +664,7 @@ template <class G> __device__ __forceinline__ void jit_hot_flush(const KernelArg
         case ACC_MAX_I128: atomic_minmax_i128(dst, mk128(w0, w1), false); break;
         case ACC_MIN_F64: atomic_minmax_f64(dst, __longlong_as_double((long long)w0), true); break;
         case ACC_MAX_F64: atomic_minmax_f64(dst, __longlong_as_double((long long)w0), false); break;
+        case ACC_DD_SUM: case ACC_DD_SQ: atomic_add_dd(dst, __longlong_as_double((long long)w0), __longlong_as_double((long long)w1)); break;
         default: break;
       }
     }

@@ -17,8 +17,9 @@ inline int grid_cap(int per_sm) {
 }
 
 struct AggOutCol {
-  int32_t kind;        // 0 group key i, 1 accumulator state/final j, 2 avg(sum acc j, count acc k)
-  int32_t a, b;
+  int32_t kind;        // 0 group key i, 1 accumulator state/final j, 2 avg(sum acc j, count acc k), 3-5 variance (compiler.hpp AggOutSpec)
+  int32_t a, b, c;
+  int32_t var;         // kind 5: VAR_POP | VAR_SQRT
   int32_t width;
   int32_t src_words;
   int32_t key_word;

@@ -216,6 +216,7 @@ __device__ __noinline__ void vm_cvt(const VmInst& I, int dkind, const TileCtx& c
       case SRC_I64: iv = lds<int64_t>(p); break;
       case SRC_I128: iv = lds<i128>(p); break;
       case SRC_B: iv = lds<uint8_t>(p) ? 1 : 0; break;
+      case SRC_U64: iv = (i128)lds<uint64_t>(p); break;
       case SRC_F32: fv = lds<float>(p); isf = true; break;
       case SRC_F64: fv = lds<double>(p); isf = true; break;
     }
@@ -223,7 +224,7 @@ __device__ __noinline__ void vm_cvt(const VmInst& I, int dkind, const TileCtx& c
       case K_I32: sts<int32_t>(pd + r * 4, isf ? (int32_t)fv : (int32_t)iv); break;
       case K_I64: sts<int64_t>(pd + r * 8, isf ? (int64_t)fv : (int64_t)iv); break;
       case K_I128: sts<i128>(pd + r * 16, isf ? (i128)(int64_t)fv : iv); break;
-      case K_F64: sts<double>(pd + r * 8, isf ? fv : (I.aux == SRC_I128 ? (double)iv : (double)(int64_t)iv)); break;
+      case K_F64: sts<double>(pd + r * 8, isf ? fv : (I.aux == SRC_I128 || I.aux == SRC_U64 ? (double)iv : (double)(int64_t)iv)); break;
       case K_B: pd[r] = isf ? (fv != 0.0) : (iv != 0); break;
     }
   }
@@ -847,6 +848,12 @@ __device__ __forceinline__ uint64_t hash_packed_key(const AggParams& A, const Ke
 }
 
 
+// a variance accumulator's term travels as a double-double: high part in f, low part in the low word of i
+__device__ __forceinline__ void set_dd_value(AccVal& v, int op, double x, double n, double mean, bool merging) {
+  double h, l;
+  dd_term(op, x, n, mean, merging, h, l);
+  v.f = h; v.i = (i128)(uint64_t)__double_as_longlong(l);
+}
 __device__ __forceinline__ AccVal load_acc_value(const AccDesc& d, const TileCtx& c, int r) {
   AccVal v; v.i = 0; v.f = 0.0; v.valid = true;
   if (d.valid_slot != NO_SLOT) v.valid = c.arena[eff(c, d.valid_slot) + r] != 0;
@@ -859,6 +866,12 @@ __device__ __forceinline__ AccVal load_acc_value(const AccDesc& d, const TileCtx
     case K_F64: v.f = lds<double>(p); break;
     case K_B: v.i = *p; break;
     default: break;
+  }
+  if (acc_is_dd(d.op)) {
+    const bool merging = d.n_slot != NO_SLOT;
+    const double n = merging ? lds<double>(c.arena + eff(c, d.n_slot) + r * 8) : 0.0;
+    const double mean = merging ? lds<double>(c.arena + eff(c, d.mean_slot) + r * 8) : 0.0;
+    set_dd_value(v, d.op, v.f, n, mean, merging);
   }
   return v;
 }
@@ -880,6 +893,7 @@ __device__ __forceinline__ void acc_global(uint64_t* e, const AggParams& A, int 
     case ACC_MAX_I128: atomic_minmax_i128(w, v.i, false); break;
     case ACC_MIN_F64: atomic_minmax_f64(w, v.f, true); break;
     case ACC_MAX_F64: atomic_minmax_f64(w, v.f, false); break;
+    case ACC_DD_SUM: case ACC_DD_SQ: atomic_add_dd(w, v.f, __longlong_as_double((long long)(uint64_t)v.i)); break;
     default: break;
   }
   if (d.track_seen) {
@@ -1089,6 +1103,12 @@ __device__ __forceinline__ void sink_agg(const PipelineParams& P, const AggParam
                 default: vi[k] = *p;
               }
             }
+            if (acc_is_dd(d.op)) {
+              const bool merging = d.n_slot != NO_SLOT;
+              AccVal t;
+              set_dd_value(t, d.op, vf[k], merging ? lds<double>(c.arena + d.n_slot + r * 8) : 0.0, merging ? lds<double>(c.arena + d.mean_slot + r * 8) : 0.0, merging);
+              vf[k] = t.f; vi[k] = t.i;
+            }
             if (d.op == ACC_SUM_I128 && ok[k] && !fits55(vi[k])) {   // rare: exact value straight to the table
               uint64_t* e = hot_entry(P, A, H, gid[k]);
               if (e) { atomic_add_i128(e + 2 + A.key_words + d.word, vi[k]); if (d.track_seen) atomicOr(reinterpret_cast<unsigned long long*>(e + 1), 1ull << j); }
@@ -1132,14 +1152,14 @@ __device__ __forceinline__ void sink_agg(const PipelineParams& P, const AggParam
               if (lane == 0) slot[0] = (uint64_t)__double_as_longlong(__longlong_as_double((long long)slot[0]) + part);
               break;
             }
-            default: {   // min / max: serial over member lanes through lane 0 (rarely hot)
+            default: {   // min / max (rarely hot) and the double-double sums: per thread, then a shuffle tree, then lane 0
               uint64_t w0 = acc_identity(d.op, 0), w1 = acc_identity(d.op, 1);
 #pragma unroll
               for (int k = 0; k < RPT; ++k) {
                 if (ok[k] && gid[k] == g) {
-                  const bool isf = d.op == ACC_MIN_F64 || d.op == ACC_MAX_F64;
+                  const bool isf = d.op == ACC_MIN_F64 || d.op == ACC_MAX_F64 || acc_is_dd(d.op);
                   const uint64_t v0 = isf ? (uint64_t)__double_as_longlong(vf[k]) : (uint64_t)(u128)vi[k];
-                  const uint64_t v1 = isf ? 0 : (uint64_t)((u128)vi[k] >> 64);
+                  const uint64_t v1 = acc_is_dd(d.op) ? (uint64_t)(u128)vi[k] : isf ? 0 : (uint64_t)((u128)vi[k] >> 64);
                   acc_combine_words(d.op, w0, w1, v0, v1);
                 }
               }
@@ -1404,6 +1424,7 @@ __device__ __forceinline__ void hot_flush(const PipelineParams& P, const AggPara
       case ACC_MAX_I128: atomic_minmax_i128(dst, (i128)(((u128)w1 << 64) | w0), false); break;
       case ACC_MIN_F64: atomic_minmax_f64(dst, __longlong_as_double((long long)w0), true); break;
       case ACC_MAX_F64: atomic_minmax_f64(dst, __longlong_as_double((long long)w0), false); break;
+      case ACC_DD_SUM: case ACC_DD_SQ: atomic_add_dd(dst, __longlong_as_double((long long)w0), __longlong_as_double((long long)w1)); break;
       default: break;
     }
   }
@@ -1944,6 +1965,32 @@ __global__ void agg_migrate_kernel(AggParams A, AggMigrateMap M, const uint8_t* 
   }
 }
 
+// The variance family's state from a count n and double-double sums S = sum x and Q = sum x^2: mean = S / n and
+// m2 = Q - S^2 / n, both formed in double-double and rounded once.  An m2 within the rounding error of those sums of zero
+// (n * Q * 2^-100) is 0: equal values give exactly 0, and the negative values cancellation could leave never appear.  NaN,
+// from a NaN or infinite value or from a square beyond the Float64 range, stays NaN.  n = 0 gives 0 and 0.
+__device__ __forceinline__ void variance_moments(double n, double sh, double sl, double qh, double ql, bool want_m2, double* mean, double* m2) {
+  if (n == 0.0) { *mean = 0.0; *m2 = 0.0; return; }
+  // S / n
+  const double q1 = sh / n;
+  double rh = sh, rl = sl;
+  { const double p = q1 * n; dd_add(rh, rl, -p, -fma(q1, n, -p)); }
+  *mean = q1 + (rh + rl) / n;
+  if (!want_m2) return;
+  // S^2 / n
+  double s2h, s2l;
+  { const double p = sh * sh; dd_fast_two_sum(p, fma(sh, sh, -p) + 2.0 * sh * sl, s2h, s2l); }
+  const double d1 = s2h / n;
+  double eh = s2h, el = s2l;
+  { const double p = d1 * n; dd_add(eh, el, -p, -fma(d1, n, -p)); }
+  double dh, dl;
+  dd_fast_two_sum(d1, (eh + el) / n, dh, dl);
+  double mh = qh, ml = ql;
+  dd_add(mh, ml, -dh, -dl);
+  const double v = mh + ml;
+  *m2 = v <= fabs(qh) * n * 0x1p-100 ? 0.0 : v;
+}
+
 __global__ void agg_extract_kernel(AggParams A, AggExtractParams X, uint64_t n_groups, uint32_t* err) {
   for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n_groups; i += (uint64_t)gridDim.x * blockDim.x) {
     const uint64_t* e = reinterpret_cast<const uint64_t*>(A.table) + (uint64_t)A.occ[i] * A.entry_words;
@@ -1977,6 +2024,21 @@ __global__ void agg_extract_kernel(AggParams A, AggExtractParams X, uint64_t n_g
         else if (o.width == 4) *reinterpret_cast<uint32_t*>(dst) = valid ? (uint32_t)s[0] : 0;
         else if (o.width == 2) *reinterpret_cast<uint16_t*>(dst) = valid ? (uint16_t)s[0] : 0;
         else *dst = valid ? (uint8_t)s[0] : 0;
+      } else if (o.kind >= 3) {
+        const uint64_t cnt = aw[A.accs[o.b].word];
+        double mean, m2;
+        const uint64_t* sw = aw + A.accs[o.kind == 3 ? o.a : o.c].word;
+        const uint64_t* qw = aw + A.accs[o.a].word;
+        variance_moments((double)cnt, __longlong_as_double((long long)sw[0]), __longlong_as_double((long long)sw[1]),
+                         __longlong_as_double((long long)qw[0]), __longlong_as_double((long long)qw[1]), o.kind == 4 || o.kind == 5, &mean, &m2);
+        double x = o.kind == 3 ? mean : m2;
+        if (o.kind == 5) {
+          const bool pop = o.var & VAR_POP;
+          valid = pop ? cnt >= 1 : cnt >= 2;
+          x = valid ? m2 / (double)(pop ? cnt : cnt - 1) : 0.0;
+          if (o.var & VAR_SQRT) x = sqrt(x);
+        }
+        *reinterpret_cast<double*>(dst) = x;
       } else {
         const AccDesc& ds = A.accs[o.a];
         const uint64_t cnt = aw[A.accs[o.b].word];

@@ -201,7 +201,10 @@ struct PipelineRunner {
         A = *aux_host;
         for (int i = 0; i < A.agg.n_keys; ++i) rs_key(A.agg.keys[i], add);
         for (int w = 0; w < A.agg.key_words; ++w) { A.agg.kwords[w].slot = rs(A.agg.kwords[w].slot, add); A.agg.kwords[w].valid_slot = rs(A.agg.kwords[w].valid_slot, add); }
-        for (int j = 0; j < A.agg.n_accs; ++j) { A.agg.accs[j].value_slot = rs(A.agg.accs[j].value_slot, add); A.agg.accs[j].valid_slot = rs(A.agg.accs[j].valid_slot, add); }
+        for (int j = 0; j < A.agg.n_accs; ++j) {
+          AccDesc& d = A.agg.accs[j];
+          d.value_slot = rs(d.value_slot, add); d.valid_slot = rs(d.valid_slot, add); d.n_slot = rs(d.n_slot, add); d.mean_slot = rs(d.mean_slot, add);
+        }
         for (int j = 0; j < A.agg.n_accs && j < REG_ACCS; ++j) if (A.agg.rload[j].mode) A.agg.rload[j].slot = rs(A.agg.rload[j].slot, add);
         for (int i = 0; i < A.build.n_keys; ++i) rs_key(A.build.keys[i], add);
         for (int i = 0; i < A.part.n_keys; ++i) rs_key(A.part.keys[i], add);

@@ -68,7 +68,7 @@ enum VmBase : uint16_t {
 enum TsPart : uint16_t { TS_YEAR = 0, TS_QUARTER, TS_MONTH, TS_WEEK, TS_DAY, TS_HOUR, TS_MINUTE, TS_SECOND, TS_DAYS };
 enum : uint16_t { F_IMM_A = 1, F_IMM_B = 2 };
 // OP_CVT source formats (aux)
-enum CvtSrc : uint16_t { SRC_I8 = 0, SRC_I16, SRC_U8, SRC_U16, SRC_U32, SRC_F32, SRC_I32, SRC_I64, SRC_F64, SRC_I128, SRC_B };
+enum CvtSrc : uint16_t { SRC_I8 = 0, SRC_I16, SRC_U8, SRC_U16, SRC_U32, SRC_F32, SRC_I32, SRC_I64, SRC_F64, SRC_I128, SRC_B, SRC_U64 };
 enum LikeClass : uint16_t { LIKE_EXACT = 0, LIKE_PREFIX = 1, LIKE_SUFFIX = 2, LIKE_CONTAINS = 3, LIKE_GENERIC = 4 };
 
 struct VmInst {
@@ -105,8 +105,13 @@ enum AccOp : uint8_t {
   ACC_SUM_F64,
   ACC_COUNT,         // state i64 += 1 when value valid (or always when value slot == NO_SLOT)
   ACC_MIN_I64, ACC_MAX_I64, ACC_MIN_I128, ACC_MAX_I128, ACC_MIN_F64, ACC_MAX_F64,
-  ACC_MIN_I32, ACC_MAX_I32
+  ACC_MIN_I32, ACC_MAX_I32,
+  // variance family: double-double sums (word 0 the high double, word 1 the low one), updated by a 16-byte compare-and-swap
+  ACC_DD_SUM,        // state += x                        (merging: += count * mean, formed exactly)
+  ACC_DD_SQ          // state += x * x, formed exactly    (merging: += m2 + count * mean^2)
 };
+__host__ __device__ constexpr bool acc_is_dd(int op) { return op == ACC_DD_SUM || op == ACC_DD_SQ; }
+enum : int { VAR_POP = 1, VAR_SQRT = 2 };   // variance outputs: divide by n (else n - 1); take the square root
 
 struct AccDesc {
   uint8_t op;
@@ -116,6 +121,8 @@ struct AccDesc {
   uint32_t value_slot;     // NO_SLOT for count(*)
   uint32_t valid_slot;     // NO_SLOT => never null
   uint16_t word;           // first 8-byte word of this accumulator inside a global table entry
+  uint32_t n_slot;         // ACC_DD_* merging a state row: F64 slots of its count and mean (stride 8); NO_SLOT otherwise
+  uint32_t mean_slot;
 };
 
 // One 8-byte word of the packed group key: where it is loaded from (static indexing => registers).

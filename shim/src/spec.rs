@@ -132,7 +132,8 @@ pub fn aggregate(a: &AggregateExec) -> Option<Value> {
     for f in a.aggr_expr() {
         if !f.order_bys().is_empty() { return None; }
         let fun = f.fun().name().to_lowercase();
-        if !matches!(fun.as_str(), "sum" | "avg" | "count" | "min" | "max") { return None; }
+        // the variance family under DataFusion's physical names (stddev / var are the sample forms); aliases stay on the CPU
+        if !matches!(fun.as_str(), "sum" | "avg" | "count" | "min" | "max" | "stddev" | "stddev_pop" | "var" | "var_pop") { return None; }
         // DISTINCT over one argument of a single-mode aggregate; in a partial / final pair its state is a List column, and such
         // a pair stays a DataFusion node
         let distinct = f.is_distinct();
