@@ -589,9 +589,7 @@ void PipelineCompiler::finalize(CompiledPipeline& out, Ctx* ctx, int hot_wanted)
   const size_t fixed = 256;
   SG_CHECK(prog_.size() <= (size_t)MAX_INST, SAILGPU_ERR_UNSUPPORTED, "fused pipeline needs more than " + std::to_string(MAX_INST) + " VM instructions");
   const AggParams& A = out.agg;
-  // per hot group: key words + fingerprint + entry pointer + one accumulator block per warp
-  const size_t per_group = out.sink == SINK_AGG ? (size_t)HOT_KEY_WORDS * 8 + 16 + 32 + (size_t)(NT / 32) * (1 + 2 * A.n_accs) * 8 : 0;
-  if (out.sink == SINK_AGG && A.key_words > HOT_KEY_WORDS) hot_wanted = 0;
+  if (out.sink != SINK_AGG || A.key_words > HOT_KEY_WORDS) hot_wanted = 0;
   auto layout = [&](int rpt, int stages, uint32_t* temps, uint32_t* stage) {
     const uint32_t tile = (uint32_t)rpt * NT;
     uint32_t t = 0, s = 0;
@@ -627,6 +625,7 @@ void PipelineCompiler::finalize(CompiledPipeline& out, Ctx* ctx, int hot_wanted)
                           : out.sink == SINK_STORE ? C_STORE : latency_bound ? C_AGG_COLD : C_OTHER;
   int best_rpt = 0, best_stages = 0, best_hot = 0;
   if (hot_wanted > 0 && force_hot >= 0) hot_wanted = force_hot;
+  hot_wanted = std::min(hot_wanted, HOT_MAX_GROUPS);
   for (int pass = 0; pass < 2 && !best_rpt; ++pass) {
     // pass 0: demand the wanted number of hot groups (min 4 when grouping); pass 1: whatever fits
     for (int ci = 0; ci < 6; ++ci) {
@@ -636,9 +635,9 @@ void PipelineCompiler::finalize(CompiledPipeline& out, Ctx* ctx, int hot_wanted)
       uint32_t t, s;
       const size_t need = layout(c[0], c[1], &t, &s);
       if (need > budget) continue;
-      int hot = 0;
-      if (per_group && hot_wanted > 0) hot = (int)std::min<size_t>((size_t)hot_wanted, (budget - need) / per_group);
-      if (pass == 0 && per_group && hot_wanted > 0 && hot < std::min(hot_wanted, 4)) continue;
+      int hot = 0;       // the CTA dictionary takes what is left, up to hot_wanted groups
+      while (hot < hot_wanted && need + hot_scratch_bytes(hot + 1, A.n_accs) <= budget) ++hot;
+      if (pass == 0 && hot_wanted > 0 && hot < std::min(hot_wanted, 4)) continue;
       best_rpt = c[0]; best_stages = c[1]; best_hot = hot;
       break;
     }
@@ -649,7 +648,7 @@ void PipelineCompiler::finalize(CompiledPipeline& out, Ctx* ctx, int hot_wanted)
   layout(best_rpt, best_stages, &temps, &stage);
   const uint32_t tile = (uint32_t)best_rpt * NT;
   out.temps_bytes = temps; out.stage_bytes = stage;
-  out.hot_bytes = (uint32_t)((best_hot * per_group + 127) & ~(size_t)127) + ((out.extra_scratch + 127) & ~127u);
+  out.hot_bytes = hot_scratch_bytes(best_hot, A.n_accs) + ((out.extra_scratch + 127) & ~127u);
   out.scratch_off = temps;
   // assign offsets
   uint32_t t_off = 0, s_off = temps + out.hot_bytes;

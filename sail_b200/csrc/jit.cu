@@ -245,7 +245,7 @@ struct Emitter {
     const AggParams& A = J.agg;
     std::ostringstream o;
     const int tier = A.cold_only ? 0 : A.reg_path ? 2 : A.hot_groups > 0 ? 1 : 0;
-    const int hot_g = std::min(8, std::max(A.hot_groups, tier == 2 ? REG_GROUPS : 0));
+    const int hot_g = std::min(HOT_MAX_GROUPS, std::max(A.hot_groups, tier == 2 ? REG_GROUPS : 0));
     std::vector<int> ops, words, seen, modes;
     for (int j = 0; j < A.n_accs; ++j) {
       ops.push_back(A.accs[j].op); words.push_back(A.accs[j].word); seen.push_back(A.accs[j].track_seen);
@@ -442,8 +442,8 @@ bool jit_plan(const CompiledPipeline& cp, size_t max_smem, JitPlan* plan) {
   if (cp.sink == SINK_AGG) {
     const AggParams& A = J.agg;
     const int tier = A.cold_only ? 0 : A.reg_path ? 2 : A.hot_groups > 0 ? 1 : 0;
-    const int hot_g = std::min(8, std::max(A.hot_groups, tier == 2 ? REG_GROUPS : 0));
-    if (tier > 0) p.scratch_bytes = align128((uint32_t)(32 + hot_g * (HOT_KEY_WORDS * 8 + 8) + (NT / 32) * hot_g * (1 + 2 * A.n_accs) * 8));
+    const int hot_g = std::min(HOT_MAX_GROUPS, std::max(A.hot_groups, tier == 2 ? REG_GROUPS : 0));
+    if (tier > 0) p.scratch_bytes = hot_scratch_bytes(hot_g, A.n_accs);
     target = tier == 0 ? 3 : 2; cap = tier == 0 ? 4 : 2;
     // dictionary / register tiers: two stages streamed faster than three or four on H100 (DESIGN.md section 4.1)
     if (tier > 0) max_s = 2;

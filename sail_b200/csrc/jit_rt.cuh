@@ -11,14 +11,12 @@
 // Same operator semantics as pipeline.cu (reference: DataFusion FilterExec / ProjectionExec / AggregateExec as driven by
 // crates/sail-execution/src/job_runner.rs:64); the two kernels share the group-table layout and can serve one operator.
 #pragma once
-#include "dev_ops.cuh"
+#include "agg_hot.cuh"
 
 namespace sg {
 
-// A group key in registers: the packed key words, padded with zeros to HOT_KEY_WORDS (G::Key, jit.cu).  Indexed only by
-// constants and passed by value, so that it stays in registers -- never a local-memory array.
-template <int N> struct JitKey { uint64_t w[N]; };
-using JitHotKey = JitKey<HOT_KEY_WORDS>;
+// G::Key (jit.cu): the packed key words in registers, padded with zeros to HOT_KEY_WORDS in the dictionary tiers
+template <int N> using JitKey = KeyWords<N>;
 
 template <int I> struct IC { static constexpr int value = I; __device__ constexpr operator int() const { return I; } };
 template <int I, int N, class F> __device__ __forceinline__ void static_for(F&& f) {
@@ -43,17 +41,8 @@ constexpr long long JIT_PARTIAL = 1ll << 62;
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ uint32_t lds_acquire_u32(const uint32_t* p) {
-  uint32_t v;
-  asm volatile("ld.acquire.cta.shared.u32 %0, [%1];" : "=r"(v) : "r"(smem_u32(p)) : "memory");
-  return v;
-}
-__device__ __forceinline__ void sts_release_u32(uint32_t* p, uint32_t v) {
-  asm volatile("st.release.cta.shared.u32 [%0], %1;" ::"r"(smem_u32(p)), "r"(v) : "memory");
-}
 
 // ---- expression helpers (one call per generated statement) --------------------------------------
-__device__ __forceinline__ i128 mk128(uint64_t lo, uint64_t hi) { return (i128)(((u128)hi << 64) | lo); }
 __device__ __forceinline__ ulonglong2 mkv16(uint64_t lo, uint64_t hi) { ulonglong2 v; v.x = lo; v.y = hi; return v; }
 __device__ __forceinline__ i128 jit_mulw(int64_t a, int64_t b) {
   return mk128((unsigned long long)a * (unsigned long long)b, (unsigned long long)__mul64hi((long long)a, (long long)b));
@@ -103,8 +92,6 @@ __device__ __noinline__ bool jit_like(ulonglong2 v, const uint8_t* pat, uint32_t
   for (int i = 0; i < 8; ++i) tmp[4 + i] = (uint8_t)(v.y >> (8 * i));
   return like_match(tmp, len, pat, plen, cls);
 }
-__device__ __forceinline__ uint64_t i128_lo(i128 v) { return (uint64_t)(u128)v; }
-__device__ __forceinline__ uint64_t i128_hi(i128 v) { return (uint64_t)((u128)v >> 64); }
 
 // ================================================================================================
 // global group table (layout and protocol of pipeline.cu::agg_find_or_insert, constants from G)
@@ -172,116 +159,8 @@ __device__ __forceinline__ uint64_t* jit_find_or_insert_warp(const AggParams& A,
   return need ? got : nullptr;
 }
 
-// one accumulator update on a global table entry
-template <class G, int J>
-__device__ __forceinline__ void jit_acc_global(uint64_t* e, const AccVal& v) {
-  constexpr int op = G::acc_op(J);
-  uint64_t* w = e + 2 + G::KEY_WORDS + G::acc_word(J);
-  if constexpr (op == ACC_COUNT) { if (v.valid) atomicAdd(reinterpret_cast<unsigned long long*>(w), 1ull); return; }
-  if (!v.valid) return;
-  if constexpr (op == ACC_SUM_I64) atomicAdd(reinterpret_cast<unsigned long long*>(w), (unsigned long long)(int64_t)v.i);
-  else if constexpr (op == ACC_SUM_I128) atomic_add_i128(w, v.i);
-  else if constexpr (op == ACC_SUM_F64) atomicAdd(reinterpret_cast<double*>(w), v.f);
-  else if constexpr (op == ACC_MIN_I32 || op == ACC_MIN_I64) atomicMin(reinterpret_cast<long long*>(w), (long long)(int64_t)v.i);
-  else if constexpr (op == ACC_MAX_I32 || op == ACC_MAX_I64) atomicMax(reinterpret_cast<long long*>(w), (long long)(int64_t)v.i);
-  else if constexpr (op == ACC_MIN_I128) atomic_minmax_i128(w, v.i, true);
-  else if constexpr (op == ACC_MAX_I128) atomic_minmax_i128(w, v.i, false);
-  else if constexpr (op == ACC_MIN_F64) atomic_minmax_f64(w, v.f, true);
-  else if constexpr (op == ACC_MAX_F64) atomic_minmax_f64(w, v.f, false);
-  else if constexpr (acc_is_dd(op)) atomic_add_dd(w, v.f, __longlong_as_double((long long)i128_lo(v.i)));
-  if constexpr (G::acc_seen(J) != 0) {
-    const unsigned long long bit = 1ull << J;
-    if (!(*reinterpret_cast<volatile unsigned long long*>(e + 1) & bit)) atomicOr(reinterpret_cast<unsigned long long*>(e + 1), bit);
-  }
-}
-
-// ================================================================================================
-// CTA dictionary of hot groups (shared memory).  Entries are immutable once published; dict_n is
-// released after the entry is written, so readers need no lock.  Growth takes a CTA-wide spin lock,
-// one lane per warp at a time.
-// ================================================================================================
-struct JitHot { uint32_t* fp32; uint64_t* keys; uint64_t* entry; uint64_t* wacc; };
-template <class G> __device__ __forceinline__ JitHot jit_hot(uint8_t* scratch) {
-  JitHot h;
-  uint8_t* p = scratch;
-  h.fp32 = reinterpret_cast<uint32_t*>(p); p += 32;
-  h.keys = reinterpret_cast<uint64_t*>(p); p += (size_t)G::HOT_G * HOT_KEY_WORDS * 8;
-  h.entry = reinterpret_cast<uint64_t*>(p); p += (size_t)G::HOT_G * 8;
-  h.wacc = reinterpret_cast<uint64_t*>(p);
-  return h;
-}
-template <class G> constexpr int jit_aw() { return 1 + 2 * G::N_ACCS; }     // per (warp, group): seen word + {lo, hi} per accumulator
-
-__device__ __forceinline__ uint32_t jit_fp(const JitHotKey& kw) {
-  uint32_t fp = fold32(kw.w[0]);
-  fp = __funnelshift_l(fp, fp, 7) ^ fold32(kw.w[1]);
-  fp = __funnelshift_l(fp, fp, 7) ^ fold32(kw.w[2]);
-  fp = __funnelshift_l(fp, fp, 7) ^ fold32(kw.w[3]);
-  return fp;
-}
-__device__ __forceinline__ bool jit_dict_verify(const JitHot& H, int g, const JitHotKey& kw) {
-  const ulonglong2* hk = reinterpret_cast<const ulonglong2*>(H.keys + g * HOT_KEY_WORDS);
-  const ulonglong2 a = hk[0], b = hk[1];
-  return ((a.x ^ kw.w[0]) | (a.y ^ kw.w[1]) | (b.x ^ kw.w[2]) | (b.y ^ kw.w[3])) == 0ull;
-}
-template <int CAP>
-__device__ __forceinline__ int jit_dict_lookup(const JitHot& H, int n, const JitHotKey& kw, uint32_t fp) {
-  const uint4 f0 = *reinterpret_cast<const uint4*>(H.fp32);
-  if (n > 0 && f0.x == fp && jit_dict_verify(H, 0, kw)) return 0;
-  if (n > 1 && f0.y == fp && jit_dict_verify(H, 1, kw)) return 1;
-  if (n > 2 && f0.z == fp && jit_dict_verify(H, 2, kw)) return 2;
-  if (n > 3 && f0.w == fp && jit_dict_verify(H, 3, kw)) return 3;
-  if constexpr (CAP > 4) {
-    const uint4 f1 = *reinterpret_cast<const uint4*>(H.fp32 + 4);
-    if (n > 4 && f1.x == fp && jit_dict_verify(H, 4, kw)) return 4;
-    if (n > 5 && f1.y == fp && jit_dict_verify(H, 5, kw)) return 5;
-    if (n > 6 && f1.z == fp && jit_dict_verify(H, 6, kw)) return 6;
-    if (n > 7 && f1.w == fp && jit_dict_verify(H, 7, kw)) return 7;
-  }
-  return -1;
-}
-// warp-collective: lanes with `want` find their key in the dictionary or append it while there is room (CAP entries);
-// returns the group id or -1 (dictionary full).  Out of line (it runs while the dictionary grows), so H and the key are
-// passed by value: a reference would keep them in local memory in the caller, stored on every tile.
-template <int CAP>
-__device__ __noinline__ int jit_dict_add(JitSmem* sm, const JitHot H, bool want, const JitHotKey kw, uint32_t fp) {
-  const int lane = threadIdx.x & 31;
-  int g = -1;
-  bool gave_up = false;
-  for (;;) {
-    const bool need = want && g < 0 && !gave_up;
-    const unsigned pend = __ballot_sync(0xFFFFFFFFu, need);
-    if (!pend) break;
-    const int leader = __ffs(pend) - 1;
-    if (lane == leader) {
-      while (atomicCAS(&sm->dict_lock, 0u, 1u) != 0u) __nanosleep(20);
-      const int n = (int)lds_acquire_u32(&sm->dict_n);
-      g = jit_dict_lookup<CAP>(H, n, kw, fp);
-      if (g < 0) {
-        if (n < CAP) {
-#pragma unroll
-          for (int w = 0; w < HOT_KEY_WORDS; ++w) H.keys[n * HOT_KEY_WORDS + w] = kw.w[w];
-          H.fp32[n] = fp;
-          H.entry[n] = 0;
-          sts_release_u32(&sm->dict_n, (uint32_t)(n + 1));
-          g = n;
-        } else gave_up = true;
-      }
-      __threadfence_block();
-      atomicExch(&sm->dict_lock, 0u);
-    }
-    __syncwarp();
-    if (need && lane != leader) {
-      const int n = (int)lds_acquire_u32(&sm->dict_n);
-      g = jit_dict_lookup<CAP>(H, n, kw, fp);
-      if (g < 0 && n >= CAP) gave_up = true;
-    }
-  }
-  return g;
-}
-
 template <class G>
-__device__ __noinline__ uint64_t* jit_hot_entry(const KernelArgs& K, const JitHot H, int g) {
+__device__ __noinline__ uint64_t* jit_hot_entry(const KernelArgs& K, const HotDict H, int g) {
   uint64_t* e = reinterpret_cast<uint64_t*>(*reinterpret_cast<volatile uint64_t*>(H.entry + g));
   if (e) return e;
   typename G::Key kw;
@@ -320,9 +199,8 @@ __device__ __forceinline__ void jit_acc_merge(AccVal& a, const AccVal& b) {
 template <class G, int J>
 __device__ __forceinline__ void jit_acc_global_n(uint64_t* e, const AccVal& v) {
   constexpr int op = G::acc_op(J);
-  if constexpr (op == ACC_COUNT) {
-    if (v.valid && (int64_t)v.i != 0) atomicAdd(reinterpret_cast<unsigned long long*>(e + 2 + G::KEY_WORDS + G::acc_word(J)), (unsigned long long)(int64_t)v.i);
-  } else jit_acc_global<G, J>(e, v);
+  if constexpr (op == ACC_COUNT) { if (v.valid) acc_apply(op, e + 2 + G::KEY_WORDS + G::acc_word(J), i128_lo(v.i), 0); }
+  else acc_global(e, G::KEY_WORDS, op, G::acc_word(J), J, G::acc_seen(J) != 0, v);
 }
 
 // rows whose group is not in the dictionary (or every row of the high-cardinality variant): global table
@@ -358,7 +236,9 @@ __device__ __forceinline__ void jit_cold_rows(const KernelArgs& K, const typenam
       const int leader = __ffs(peers) - 1;
       const bool solo = peers == (1u << lane);
       if (__all_sync(0xFFFFFFFFu, solo)) {
-        if (upd) static_for<0, G::N_ACCS>([&](auto Jc) { constexpr int J = decltype(Jc)::value; jit_acc_global<G, J>(e, G::template acc<J>(rows[k])); });
+        if (upd) static_for<0, G::N_ACCS>([&](auto Jc) { constexpr int J = decltype(Jc)::value;
+          acc_global(e, G::KEY_WORDS, G::acc_op(J), G::acc_word(J), J, G::acc_seen(J) != 0, G::template acc<J>(rows[k]));
+        });
       } else {
         static_for<0, G::N_ACCS>([&](auto Jc) { constexpr int J = decltype(Jc)::value;
           AccVal v = G::template acc<J>(rows[k]);
@@ -380,51 +260,13 @@ __device__ __forceinline__ void jit_cold_rows(const KernelArgs& K, const typenam
 }
 
 // per-thread register partials of the integer fast path (tier 2)
-template <class G> struct JitAggRegs { int64_t v[REG_GROUPS][G::N_ACCS > 0 ? G::N_ACCS : 1]; int rows; };
-
-// Warp-collective (full-mask shuffles): nothing in here may depend on the dictionary size, which other warps change
-// asynchronously -- every register group is flushed, groups that do not exist yet hold zeros.
-template <class G>
-__device__ __forceinline__ void jit_reg_flush(const JitHot& H, JitAggRegs<G>& R) {
-  const int lane = threadIdx.x & 31;
-#pragma unroll
-  for (int g = 0; g < REG_GROUPS; ++g) {
-    {
-      uint64_t* wa = H.wacc + (size_t)g * jit_aw<G>();
-#pragma unroll
-      for (int j = 0; j < G::N_ACCS; ++j) {
-        const int64_t part = R.v[g][j];
-        unsigned long long lo = (unsigned long long)part;
-        long long hi = part >> 63;
-#pragma unroll
-        for (int d = 16; d; d >>= 1) {
-          const unsigned long long olo = __shfl_xor_sync(0xFFFFFFFFu, lo, d);
-          const long long ohi = __shfl_xor_sync(0xFFFFFFFFu, hi, d);
-          const unsigned long long s = lo + olo;
-          hi += ohi + (s < lo ? 1 : 0);
-          lo = s;
-        }
-        if (lane == 0 && (lo | (unsigned long long)hi)) {
-          unsigned long long* dst = reinterpret_cast<unsigned long long*>(wa + 1 + 2 * j);
-          const unsigned long long old = atomicAdd(dst, lo);
-          const unsigned long long carry = (old + lo) < old ? 1ull : 0ull;
-          const unsigned long long h2 = (unsigned long long)hi + carry;
-          if (h2) atomicAdd(dst + 1, h2);
-        }
-        R.v[g][j] = 0;
-      }
-    }
-  }
-  R.rows = 0;
-}
-
-constexpr int JIT_REG_FLUSH = 224;
+template <class G> using JitAggRegs = RegAcc<(G::N_ACCS > 0 ? G::N_ACCS : 1)>;
 
 // tier 2: counts / integer / decimal sums, first REG_GROUPS groups in registers
 template <class G>
 __device__ __forceinline__ void jit_agg_reg_tile(const KernelArgs& K, const typename G::Row (&rows)[G::RPT], JitSmem* sm, uint8_t* scratch, JitAggRegs<G>& R) {
-  static_assert(sizeof(typename G::Key) == sizeof(JitHotKey), "dictionary tiers hold keys of at most HOT_KEY_WORDS words");
-  const JitHot H = jit_hot<G>(scratch);
+  static_assert(sizeof(typename G::Key) == sizeof(HotKey), "dictionary tiers hold keys of at most HOT_KEY_WORDS words");
+  const HotDict H = hot_dict(scratch, G::HOT_G);
   int gid[G::RPT];
   uint32_t fpv[G::RPT];
   bool miss = false;
@@ -437,8 +279,8 @@ __device__ __forceinline__ void jit_agg_reg_tile(const KernelArgs& K, const type
     if (rows[k].live) {
       typename G::Key kw;
       G::key_words(rows[k], kw);
-      fpv[k] = jit_fp(kw);
-      gid[k] = jit_dict_lookup<REG_GROUPS>(H, n0, kw, fpv[k]);
+      fpv[k] = hot_fp(kw);
+      gid[k] = hot_lookup<REG_GROUPS>(H, n0, kw, fpv[k]);
       miss |= gid[k] < 0;
     }
   }
@@ -449,7 +291,7 @@ __device__ __forceinline__ void jit_agg_reg_tile(const KernelArgs& K, const type
       if (__any_sync(0xFFFFFFFFu, want)) {
         typename G::Key kw;
         G::key_words(rows[k], kw);
-        const int g = jit_dict_add<REG_GROUPS>(sm, H, want, kw, fpv[k]);
+        const int g = hot_dict_add<REG_GROUPS>(H, &sm->dict_n, &sm->dict_lock, REG_GROUPS, want, kw, fpv[k]);
         if (want) gid[k] = g;
       }
     }
@@ -469,9 +311,8 @@ __device__ __forceinline__ void jit_agg_reg_tile(const KernelArgs& K, const type
             else {                                               // rare: exact value straight to the table entry
               val[J] = 0;
               uint64_t* e = jit_hot_entry<G>(K, H, gid[k]);
-              // an Int64 sum has one word and is defined mod 2^64: no carry into the next accumulator
-              if constexpr (G::acc_op(J) == ACC_SUM_I64) { if (e) atomicAdd(reinterpret_cast<unsigned long long*>(e + 2 + G::KEY_WORDS + G::acc_word(J)), (unsigned long long)(int64_t)a.i); }
-              else { if (e) atomic_add_i128(e + 2 + G::KEY_WORDS + G::acc_word(J), a.i); }
+              // (an Int64 sum has one word and is defined mod 2^64: no carry into the next accumulator)
+              if (e) acc_apply(G::acc_op(J), e + 2 + G::KEY_WORDS + G::acc_word(J), i128_lo(a.i), i128_hi(a.i));
             }
           }
         }
@@ -496,7 +337,7 @@ __device__ __forceinline__ void jit_agg_reg_tile(const KernelArgs& K, const type
     }
   }
   R.rows += G::RPT;
-  if (R.rows >= JIT_REG_FLUSH) jit_reg_flush<G>(H, R);
+  if (R.rows >= REG_FLUSH) reg_flush(H, G::N_ACCS, R);
   bool anycold = false;
 #pragma unroll
   for (int k = 0; k < G::RPT; ++k) anycold |= rows[k].live && gid[k] < 0;
@@ -506,9 +347,8 @@ __device__ __forceinline__ void jit_agg_reg_tile(const KernelArgs& K, const type
 // tier 1: any accumulator mix, up to HOT_G groups, per-warp accumulators in shared memory (warp-shuffle reductions)
 template <class G>
 __device__ __forceinline__ void jit_agg_dict_tile(const KernelArgs& K, const typename G::Row (&rows)[G::RPT], JitSmem* sm, uint8_t* scratch) {
-  static_assert(sizeof(typename G::Key) == sizeof(JitHotKey), "dictionary tiers hold keys of at most HOT_KEY_WORDS words");
-  const JitHot H = jit_hot<G>(scratch);
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  static_assert(sizeof(typename G::Key) == sizeof(HotKey), "dictionary tiers hold keys of at most HOT_KEY_WORDS words");
+  const HotDict H = hot_dict(scratch, G::HOT_G);
   int gid[G::RPT];
   uint32_t fpv[G::RPT];
   bool miss = false;
@@ -519,8 +359,8 @@ __device__ __forceinline__ void jit_agg_dict_tile(const KernelArgs& K, const typ
     if (rows[k].live) {
       typename G::Key kw;
       G::key_words(rows[k], kw);
-      fpv[k] = jit_fp(kw);
-      gid[k] = jit_dict_lookup<G::HOT_G>(H, n0, kw, fpv[k]);
+      fpv[k] = hot_fp(kw);
+      gid[k] = hot_lookup<G::HOT_G>(H, n0, kw, fpv[k]);
       miss |= gid[k] < 0;
     }
   }
@@ -531,7 +371,7 @@ __device__ __forceinline__ void jit_agg_dict_tile(const KernelArgs& K, const typ
       if (__any_sync(0xFFFFFFFFu, want)) {
         typename G::Key kw;
         G::key_words(rows[k], kw);
-        const int g = jit_dict_add<G::HOT_G>(sm, H, want, kw, fpv[k]);
+        const int g = hot_dict_add<G::HOT_G>(H, &sm->dict_n, &sm->dict_lock, G::HOT_G, want, kw, fpv[k]);
         if (want) gid[k] = g;
       }
     }
@@ -542,133 +382,20 @@ __device__ __forceinline__ void jit_agg_dict_tile(const KernelArgs& K, const typ
   for (int k = 0; k < G::RPT; ++k) anyhot |= rows[k].live && gid[k] >= 0;
   if (__any_sync(0xFFFFFFFFu, anyhot)) {
     static_for<0, G::N_ACCS>([&](auto Jc) { constexpr int J = decltype(Jc)::value;
-      constexpr int op = G::acc_op(J);
       AccVal av[G::RPT];
-      bool ok[G::RPT];
 #pragma unroll
       for (int k = 0; k < G::RPT; ++k) {
-        ok[k] = false;
         av[k].i = 0; av[k].f = 0.0; av[k].valid = false;
-        if (rows[k].live && gid[k] >= 0) {
-          av[k] = G::template acc<J>(rows[k]);
-          ok[k] = av[k].valid;
-          if constexpr (op == ACC_SUM_I128) {
-            if (ok[k] && !fits55(av[k].i)) {
-              uint64_t* e = jit_hot_entry<G>(K, H, gid[k]);
-              if (e) { atomic_add_i128(e + 2 + G::KEY_WORDS + G::acc_word(J), av[k].i); if (G::acc_seen(J)) atomicOr(reinterpret_cast<unsigned long long*>(e + 1), 1ull << J); }
-              ok[k] = false;
-            }
-          }
-        }
+        if (rows[k].live && gid[k] >= 0) av[k] = G::template acc<J>(rows[k]);
       }
-      for (int g = 0; g < hot_n; ++g) {
-        uint64_t* wa = H.wacc + ((size_t)(warp * G::HOT_G + g)) * jit_aw<G>();
-        uint64_t* slot = wa + 1 + 2 * J;
-        bool any = false;
-#pragma unroll
-        for (int k = 0; k < G::RPT; ++k) any |= ok[k] && gid[k] == g;
-        if (__ballot_sync(0xFFFFFFFFu, any) == 0) continue;
-        if constexpr (op == ACC_COUNT) {
-          int cnt = 0;
-#pragma unroll
-          for (int k = 0; k < G::RPT; ++k) cnt += (ok[k] && gid[k] == g) ? 1 : 0;
-          cnt = __reduce_add_sync(0xFFFFFFFFu, cnt);
-          if (lane == 0) slot[0] += (uint64_t)cnt;
-        } else if constexpr (op == ACC_SUM_I64 || op == ACC_SUM_I128) {
-          int64_t part = 0;
-#pragma unroll
-          for (int k = 0; k < G::RPT; ++k) part += (ok[k] && gid[k] == g) ? (int64_t)av[k].i : 0;
-          part = warp_sum_i64(part);
-          if (lane == 0) {
-            if constexpr (op == ACC_SUM_I64) slot[0] += (uint64_t)part;
-            else { const uint64_t lo = slot[0] + (uint64_t)part; slot[1] += (uint64_t)(part >> 63) + (lo < slot[0] ? 1ull : 0ull); slot[0] = lo; }
-          }
-        } else if constexpr (op == ACC_SUM_F64) {
-          double part = 0.0;
-#pragma unroll
-          for (int k = 0; k < G::RPT; ++k) part += (ok[k] && gid[k] == g) ? av[k].f : 0.0;
-          part = warp_sum_f64(part);
-          if (lane == 0) slot[0] = (uint64_t)__double_as_longlong(__longlong_as_double((long long)slot[0]) + part);
-        } else {
-          uint64_t w0 = acc_identity(op, 0), w1 = acc_identity(op, 1);
-#pragma unroll
-          for (int k = 0; k < G::RPT; ++k) {
-            if (ok[k] && gid[k] == g) {
-              constexpr bool isf = op == ACC_MIN_F64 || op == ACC_MAX_F64 || acc_is_dd(op);
-              const uint64_t v0 = isf ? (uint64_t)__double_as_longlong(av[k].f) : i128_lo(av[k].i);
-              const uint64_t v1 = acc_is_dd(op) ? i128_lo(av[k].i) : isf ? 0 : i128_hi(av[k].i);
-              acc_combine_words(op, w0, w1, v0, v1);
-            }
-          }
-#pragma unroll
-          for (int dlt = 16; dlt; dlt >>= 1) {
-            const uint64_t o0 = __shfl_xor_sync(0xFFFFFFFFu, w0, dlt), o1 = __shfl_xor_sync(0xFFFFFFFFu, w1, dlt);
-            acc_combine_words(op, w0, w1, o0, o1);
-          }
-          if (lane == 0) { uint64_t a0 = slot[0], a1 = slot[1]; acc_combine_words(op, a0, a1, w0, w1); slot[0] = a0; slot[1] = a1; }
-        }
-        if (G::acc_seen(J) && lane == 0) wa[0] |= 1ull << J;
-      }
+      hot_fold<G::RPT>(H, G::HOT_G, G::N_ACCS, hot_n, G::KEY_WORDS, G::acc_op(J), G::acc_word(J), J, G::acc_seen(J) != 0, av, gid,
+                       [&](int g) { return jit_hot_entry<G>(K, H, g); });
     });
   }
   bool anycold = false;
 #pragma unroll
   for (int k = 0; k < G::RPT; ++k) anycold |= rows[k].live && gid[k] < 0;
   if (__any_sync(0xFFFFFFFFu, anycold)) jit_cold_rows<G>(K, rows, gid);
-}
-
-template <class G> __device__ __forceinline__ void jit_hot_init(uint8_t* scratch) {
-  if constexpr (G::AGG_TIER > 0) {
-    const JitHot H = jit_hot<G>(scratch);
-    for (int i = threadIdx.x; i < JIT_NWARPS * G::HOT_G; i += NT) {
-      uint64_t* wa = H.wacc + (size_t)i * jit_aw<G>();
-      wa[0] = 0;
-      static_for<0, G::N_ACCS>([&](auto Jc) { constexpr int J = decltype(Jc)::value; wa[1 + 2 * J] = acc_identity(G::acc_op(J), 0); wa[2 + 2 * J] = acc_identity(G::acc_op(J), 1); });
-    }
-  }
-}
-
-// end of kernel (after a CTA barrier): fold the per-warp accumulators of every hot group into the global table
-template <class G> __device__ __forceinline__ void jit_hot_flush(const KernelArgs& K, JitSmem* sm, uint8_t* scratch) {
-  if constexpr (G::AGG_TIER > 0) {
-    const JitHot H = jit_hot<G>(scratch);
-    const int n = (int)lds_acquire_u32(&sm->dict_n);
-    for (int g = threadIdx.x; g < n; g += NT) jit_hot_entry<G>(K, H, g);
-    __syncthreads();
-    constexpr int per = G::N_ACCS + 1;
-    for (int p = threadIdx.x; p < n * per; p += NT) {
-      const int g = p / per, j = p % per;
-      uint64_t* e = reinterpret_cast<uint64_t*>(H.entry[g]);
-      if (!e) continue;
-      if (j == G::N_ACCS) {
-        uint64_t seen = 0;
-        for (int w = 0; w < JIT_NWARPS; ++w) seen |= H.wacc[((size_t)(w * G::HOT_G + g)) * jit_aw<G>()];
-        if (seen) atomicOr(reinterpret_cast<unsigned long long*>(e + 1), (unsigned long long)seen);
-        continue;
-      }
-      const int op = G::acc_op(j);
-      uint64_t w0 = acc_identity(op, 0), w1 = acc_identity(op, 1);
-      if (op == ACC_SUM_I128) { w0 = 0; w1 = 0; }
-      for (int w = 0; w < JIT_NWARPS; ++w) {
-        const uint64_t* slot = H.wacc + ((size_t)(w * G::HOT_G + g)) * jit_aw<G>() + 1 + 2 * j;
-        acc_combine_words(op, w0, w1, slot[0], slot[1]);
-      }
-      uint64_t* dst = e + 2 + G::KEY_WORDS + G::acc_word(j);
-      switch (op) {
-        case ACC_SUM_I64: case ACC_COUNT: if (w0) atomicAdd(reinterpret_cast<unsigned long long*>(dst), (unsigned long long)w0); break;
-        case ACC_SUM_I128: atomic_add_i128(dst, mk128(w0, w1)); break;
-        case ACC_SUM_F64: atomicAdd(reinterpret_cast<double*>(dst), __longlong_as_double((long long)w0)); break;
-        case ACC_MIN_I32: case ACC_MIN_I64: atomicMin(reinterpret_cast<long long*>(dst), (long long)w0); break;
-        case ACC_MAX_I32: case ACC_MAX_I64: atomicMax(reinterpret_cast<long long*>(dst), (long long)w0); break;
-        case ACC_MIN_I128: atomic_minmax_i128(dst, mk128(w0, w1), true); break;
-        case ACC_MAX_I128: atomic_minmax_i128(dst, mk128(w0, w1), false); break;
-        case ACC_MIN_F64: atomic_minmax_f64(dst, __longlong_as_double((long long)w0), true); break;
-        case ACC_MAX_F64: atomic_minmax_f64(dst, __longlong_as_double((long long)w0), false); break;
-        case ACC_DD_SUM: case ACC_DD_SQ: atomic_add_dd(dst, __longlong_as_double((long long)w0), __longlong_as_double((long long)w1)); break;
-        default: break;
-      }
-    }
-  }
 }
 
 // ================================================================================================
@@ -792,7 +519,7 @@ __device__ __forceinline__ void jit_main(const KernelArgs& K) {
     fence_barrier_init();
     sm->dict_n = 0; sm->dict_lock = 0;
   }
-  if constexpr (G::SINK == SINK_AGG) jit_hot_init<G>(scratch);
+  if constexpr (G::SINK == SINK_AGG && G::AGG_TIER > 0) hot_init(hot_dict(scratch, G::HOT_G), G::HOT_G, G::N_ACCS, [](int j) { return G::acc_op(j); });
   __syncthreads();
 
   // ---- producer (thread 0): hands tiles to stages ------------------------------------------------
@@ -889,10 +616,11 @@ __device__ __forceinline__ void jit_main(const KernelArgs& K) {
     __syncwarp();
     if (lane == 0) mbar_arrive(&sm->empty[s]);
   }
-  if constexpr (G::SINK == SINK_AGG) {
-    if constexpr (G::AGG_TIER == 2) { const JitHot H = jit_hot<G>(scratch); jit_reg_flush<G>(H, R); }
-    __syncthreads();
-    jit_hot_flush<G>(K, sm, scratch);
+  if constexpr (G::SINK == SINK_AGG && G::AGG_TIER > 0) {
+    const HotDict H = hot_dict(scratch, G::HOT_G);
+    if constexpr (G::AGG_TIER == 2) reg_flush(H, G::N_ACCS, R);
+    hot_flush(H, &sm->dict_n, G::HOT_G, G::N_ACCS, G::KEY_WORDS, [](int j) { return G::acc_op(j); }, [](int j) { return G::acc_word(j); },
+              [&](int g) { return jit_hot_entry<G>(K, H, g); });
   }
 }
 

@@ -10,6 +10,7 @@
 
 #include <algorithm>
 
+#include "agg_hot.cuh"
 #include "dev_ops.cuh"
 #include "dev_util.cuh"
 #include "kernels.hpp"
@@ -20,8 +21,8 @@ namespace sg {
 struct Smem {
   uint64_t full[2];        // TMA "tile landed" barriers, one per stage
   int32_t tile[2];
-  int32_t hot_n;           // groups in the CTA-local hot dictionary
-  int32_t elect;
+  uint32_t dict_n;         // groups in the CTA dictionary (agg_hot.cuh; release/acquire)
+  uint32_t dict_lock;
   uint32_t cache_count;    // BUILD: occupied entries of the CTA chain cache
   int32_t defer[2];        // AGG with a bounded table: "stop taking tiles" flag, double buffered across iterations
   unsigned long long tile_base;   // COMPACT: exclusive prefix of this tile
@@ -877,87 +878,38 @@ __device__ __forceinline__ AccVal load_acc_value(const AccDesc& d, const TileCtx
 }
 
 
-// apply one accumulator update to a GLOBAL table entry (atomics)
-__device__ __forceinline__ void acc_global(uint64_t* e, const AggParams& A, int j, const AccVal& v) {
-  const AccDesc& d = A.accs[j];
-  uint64_t* w = e + 2 + A.key_words + d.word;
-  if (d.op == ACC_COUNT) { if (v.valid) atomicAdd(reinterpret_cast<unsigned long long*>(w), 1ull); return; }
-  if (!v.valid) return;
-  switch (d.op) {
-    case ACC_SUM_I64: atomicAdd(reinterpret_cast<unsigned long long*>(w), (unsigned long long)(int64_t)v.i); break;
-    case ACC_SUM_I128: atomic_add_i128(w, v.i); break;
-    case ACC_SUM_F64: atomicAdd(reinterpret_cast<double*>(w), v.f); break;
-    case ACC_MIN_I32: case ACC_MIN_I64: atomicMin(reinterpret_cast<long long*>(w), (long long)(int64_t)v.i); break;
-    case ACC_MAX_I32: case ACC_MAX_I64: atomicMax(reinterpret_cast<long long*>(w), (long long)(int64_t)v.i); break;
-    case ACC_MIN_I128: atomic_minmax_i128(w, v.i, true); break;
-    case ACC_MAX_I128: atomic_minmax_i128(w, v.i, false); break;
-    case ACC_MIN_F64: atomic_minmax_f64(w, v.f, true); break;
-    case ACC_MAX_F64: atomic_minmax_f64(w, v.f, false); break;
-    case ACC_DD_SUM: case ACC_DD_SQ: atomic_add_dd(w, v.f, __longlong_as_double((long long)(uint64_t)v.i)); break;
-    default: break;
-  }
-  if (d.track_seen) {
-    unsigned long long bit = 1ull << j;
-    if (!(*reinterpret_cast<volatile unsigned long long*>(e + 1) & bit)) atomicOr(reinterpret_cast<unsigned long long*>(e + 1), bit);
-  }
-}
-
-
-// Hot path for low-cardinality grouping (TPC-H Q1: 4 groups).  Scratch in shared memory, at
-// arena + A.hot_smem_off:
-//   u64 keys[G][key_words]     CTA-local dictionary of the first G distinct keys seen
-//   u64 fps[G]                 key fingerprints (cheap multiply-add mix) for the lookup
-//   u64 entry[G]               global table entries (resolved lazily / at flush)
-//   u64 wacc[(warp*G + g) * (1 + 2*n_accs)]   per-WARP accumulators: [seen][acc0 lo,hi][acc1 lo,hi]...
-// Every row finds its group id by fingerprint; then, accumulator by accumulator and group by
-// group, the warp reduces its rows with shuffles and lane 0 folds the warp total into wacc.  No
-// atomics, no per-thread state, ~G*n_accs*30 instructions per warp-tile regardless of tile size.
-constexpr int NWARPS = NT / 32;
-struct HotView {
-  uint32_t* fp32; uint64_t* keys; uint64_t* fps; uint64_t* entry; uint64_t* wacc; int G; int aw;
-};
-__device__ __forceinline__ HotView hot_view(const AggParams& A, uint8_t* arena) {
-  HotView h; h.G = A.hot_groups; h.aw = 1 + 2 * A.n_accs;
-  uint8_t* p = arena + A.hot_smem_off;
-  h.fp32 = reinterpret_cast<uint32_t*>(p); p += 32;                    // 8 x u32 fingerprints (register path: one LDS.128)
-  h.keys = reinterpret_cast<uint64_t*>(p); p += (size_t)h.G * HOT_KEY_WORDS * 8;
-  h.fps = reinterpret_cast<uint64_t*>(p); p += (size_t)h.G * 8;
-  h.entry = reinterpret_cast<uint64_t*>(p); p += (size_t)h.G * 8;
-  h.wacc = reinterpret_cast<uint64_t*>(p);
-  return h;
-}
-
-// packed key of row r as 8-byte words held in registers (static indexing) + its fingerprint
-__device__ __forceinline__ uint64_t pack_words(const AggParams& A, const TileCtx& c, int r, uint64_t (&kw)[HOT_KEY_WORDS]) {
+// packed key of row r as 8-byte words held in registers (static indexing), padded with zeros to HOT_KEY_WORDS
+__device__ __forceinline__ void pack_words(const AggParams& A, const TileCtx& c, int r, HotKey& kw) {
   uint64_t nullmask = 0;
-  uint64_t fp = 0x9E3779B97F4A7C15ull;
 #pragma unroll
   for (int w = 0; w < HOT_KEY_WORDS; ++w) {
-    kw[w] = 0;
+    kw.w[w] = 0;
     if (w < A.key_words && !(A.has_null_word && w == 0)) {
       const KeyWord& d = A.kwords[w];
       const uint8_t* p = c.arena + d.slot + r * d.stride + d.byte_off;
       uint64_t v = d.width == 8 ? lds<uint64_t>(p) : d.width == 4 ? (uint64_t)lds<uint32_t>(p) : (uint64_t)*p;
       if (d.valid_slot != NO_SLOT && c.arena[d.valid_slot + r] == 0) { v = 0; nullmask |= 1ull << d.key_index; }
-      kw[w] = v;
-      fp = ((fp << 9) | (fp >> 55)) ^ v;        // only a fast reject: every candidate is verified word by word
+      kw.w[w] = v;
     }
   }
-  if (A.has_null_word) { kw[0] = nullmask; fp = ((fp << 9) | (fp >> 55)) ^ nullmask; }
-  return fp;
+  if (A.has_null_word) kw.w[0] = nullmask;
 }
 
-// dictionary entries are stored padded to HOT_KEY_WORDS words, so the verify is 4 unconditional compares
-__device__ __forceinline__ int hot_lookup(const AggParams& A, const HotView& H, int hot_n, const uint64_t (&kw)[HOT_KEY_WORDS], uint64_t fp) {
-  for (int g = 0; g < hot_n; ++g) {
-    if (H.fps[g] != fp) continue;
-    const uint64_t* hk = H.keys + g * HOT_KEY_WORDS;
-    if (hk[0] == kw[0] && hk[1] == kw[1] && hk[2] == kw[2] && hk[3] == kw[3]) return g;
+// dictionary key of row r: every key word is a plain 8-byte load (views, int64, decimals) unless the plan has narrow or
+// nullable keys, in which case the general packer runs
+__device__ __forceinline__ void reg_pack(const AggParams& A, const TileCtx& c, int r, HotKey& kw) {
+  if (A.kw_simple) {
+#pragma unroll
+    for (int w = 0; w < HOT_KEY_WORDS; ++w)
+      kw.w[w] = w < A.key_words ? lds<uint64_t>(c.arena + A.kwords[w].slot + r * A.kwords[w].stride + A.kwords[w].byte_off) : 0ull;
+  } else {
+    pack_words(A, c, r, kw);
   }
-  return -1;
 }
 
-__device__ __noinline__ uint64_t* hot_entry(const PipelineParams& P, const AggParams& A, const HotView& H, int g) {
+__device__ __forceinline__ HotDict hot_dict(const AggParams& A, uint8_t* arena) { return hot_dict(arena + A.hot_smem_off, A.hot_groups); }
+
+__device__ __noinline__ uint64_t* hot_entry(const PipelineParams& P, const AggParams& A, const HotDict H, int g) {
   uint64_t* e = reinterpret_cast<uint64_t*>(H.entry[g]);
   if (e) return e;
   KeyRegs key;
@@ -993,7 +945,10 @@ __device__ __noinline__ void agg_cold_rows(const PipelineParams& P, const AggPar
       if (cold) h = pack_key<MAX_KEYS>(A.keys, A.n_keys, A.has_null_word, c, r, key, &hn);
       uint64_t* e = agg_find_or_insert_warp(A, key, h, cold, P.error_flag);
       if (cold && e) {
-        for (int j = 0; j < A.n_accs; ++j) acc_global(e, A, j, load_acc_value(A.accs[j], c, r));
+        for (int j = 0; j < A.n_accs; ++j) {
+          const AccDesc& d = A.accs[j];
+          acc_global(e, A.key_words, d.op, d.word, j, d.track_seen != 0, load_acc_value(d, c, r));
+        }
       }
     }
   }
@@ -1014,11 +969,13 @@ __device__ __forceinline__ void sink_agg_cold(const PipelineParams& P, const Agg
   agg_cold_rows<RPT>(P, A, c, gid, live);
 }
 
+// Low-cardinality grouping (TPC-H Q1: 4 groups): every row finds its group in the CTA dictionary (agg_hot.cuh); then,
+// accumulator by accumulator and group by group, the warp reduces its rows with shuffles and lane 0 folds the warp total into
+// the warp's accumulator block.  No atomics, no per-thread state, ~G*n_accs*30 instructions per warp-tile regardless of tile size.
 template <int RPT>
 __device__ __forceinline__ void sink_agg(const PipelineParams& P, const AggParams& A, const TileCtx& c, Smem* sm) {
   const uint8_t* pact = P.mask_slot == NO_SLOT ? nullptr : c.arena + P.mask_slot;
-  HotView H = hot_view(A, c.arena);
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const HotDict H = hot_dict(A, c.arena);
   int gid[RPT];
   bool live[RPT];
 #pragma unroll
@@ -1028,151 +985,49 @@ __device__ __forceinline__ void sink_agg(const PipelineParams& P, const AggParam
     gid[k] = -1;
   }
   if (A.hot_groups > 0) {
-    // phase A: look every live row up in the CTA-local dictionary
+    uint32_t fpv[RPT];
     bool miss = false;
-    const int hot_n0 = sm->hot_n;
+    // other warps grow the dictionary meanwhile: lane 0's reading is broadcast so that the warp collectives below are executed
+    // by all lanes or by none
+    const int n0 = __shfl_sync(0xFFFFFFFFu, (int)lds_acquire_u32(&sm->dict_n), 0);
 #pragma unroll
     for (int k = 0; k < RPT; ++k) {
+      fpv[k] = 0;
       if (live[k]) {
-        uint64_t kw[HOT_KEY_WORDS];
-        const uint64_t fp = pack_words(A, c, threadIdx.x + k * NT, kw);
-        gid[k] = hot_lookup(A, H, hot_n0, kw, fp);
+        HotKey kw;
+        reg_pack(A, c, threadIdx.x + k * NT, kw);
+        fpv[k] = hot_fp(kw);
+        gid[k] = hot_lookup<HOT_MAX_GROUPS>(H, n0, kw, fpv[k]);
         miss |= gid[k] < 0;
       }
     }
-    // phase B: grow the dictionary one group per round while there is room (rare after warm-up)
-    while (__syncthreads_or(miss && sm->hot_n < A.hot_groups)) {
-      if (threadIdx.x == 0) sm->elect = NT;
-      __syncthreads();
-      // (the dictionary size is read once, before the barrier: the winner appends at that index.  Reading it again next to
-      // `elect` let the compiler fetch both words with one 64-bit load in EVERY thread, which racecheck rightly reports against
-      // the winner's store -- harmless, the losers never use the value, but there is no reason to keep it)
-      const int hot_cur = sm->hot_n;
-      const bool want = miss && hot_cur < A.hot_groups;
-      if (want) atomicMin(&sm->elect, (int)threadIdx.x);
-      __syncthreads();
-      if (want && sm->elect == (int)threadIdx.x) {
-        for (int k = 0; k < RPT; ++k) {
-          if (live[k] && gid[k] < 0) {
-            uint64_t kw[HOT_KEY_WORDS];
-            const uint64_t fp = pack_words(A, c, threadIdx.x + k * NT, kw);
-            const int g = hot_cur;
-            for (int w = 0; w < HOT_KEY_WORDS; ++w) H.keys[g * HOT_KEY_WORDS + w] = kw[w];
-            H.fps[g] = fp;
-            H.entry[g] = 0;
-            sm->hot_n = g + 1;
-            break;
-          }
-        }
-      }
-      __syncthreads();
-      miss = false;
-      const int hot_n1 = sm->hot_n;
+    if (n0 < A.hot_groups && __any_sync(0xFFFFFFFFu, miss)) {
 #pragma unroll
       for (int k = 0; k < RPT; ++k) {
-        if (live[k] && gid[k] < 0) {
-          uint64_t kw[HOT_KEY_WORDS];
-          const uint64_t fp = pack_words(A, c, threadIdx.x + k * NT, kw);
-          gid[k] = hot_lookup(A, H, hot_n1, kw, fp);
-          miss |= gid[k] < 0;
+        const bool want = live[k] && gid[k] < 0;
+        if (__any_sync(0xFFFFFFFFu, want)) {
+          HotKey kw;
+          reg_pack(A, c, threadIdx.x + k * NT, kw);
+          const int g = hot_dict_add<HOT_MAX_GROUPS>(H, &sm->dict_n, &sm->dict_lock, A.hot_groups, want, kw, fpv[k]);
+          if (want) gid[k] = g;
         }
       }
     }
-    // phase C: accumulator by accumulator, group by group: thread-local partial -> warp reduce -> lane 0
-    const int hot_n = sm->hot_n;
+    const int hot_n = __shfl_sync(0xFFFFFFFFu, (int)lds_acquire_u32(&sm->dict_n), 0);      // every gid of this warp is below it
     bool anyhot = false;
 #pragma unroll
-    for (int k = 0; k < RPT; ++k) anyhot |= live[k] && gid[k] >= 0;
+    for (int k = 0; k < RPT; ++k) anyhot |= gid[k] >= 0;
     if (__any_sync(0xFFFFFFFFu, anyhot)) {
       for (int j = 0; j < A.n_accs; ++j) {
         const AccDesc& d = A.accs[j];
-        i128 vi[RPT]; double vf[RPT]; bool ok[RPT];
+        AccVal av[RPT];
 #pragma unroll
         for (int k = 0; k < RPT; ++k) {
-          vi[k] = 0; vf[k] = 0.0; ok[k] = false;
-          if (live[k] && gid[k] >= 0) {
-            const int r = threadIdx.x + k * NT;
-            ok[k] = d.valid_slot == NO_SLOT || c.arena[d.valid_slot + r] != 0;
-            if (d.value_slot != NO_SLOT) {
-              const uint8_t* p = c.arena + d.value_slot + r * d.stride;
-              switch (d.vkind) {
-                case K_I32: vi[k] = lds<int32_t>(p); break;
-                case K_I64: vi[k] = lds<int64_t>(p); break;
-                case K_I128: vi[k] = lds<i128>(p); break;
-                case K_F64: vf[k] = lds<double>(p); break;
-                default: vi[k] = *p;
-              }
-            }
-            if (acc_is_dd(d.op)) {
-              const bool merging = d.n_slot != NO_SLOT;
-              AccVal t;
-              set_dd_value(t, d.op, vf[k], merging ? lds<double>(c.arena + d.n_slot + r * 8) : 0.0, merging ? lds<double>(c.arena + d.mean_slot + r * 8) : 0.0, merging);
-              vf[k] = t.f; vi[k] = t.i;
-            }
-            if (d.op == ACC_SUM_I128 && ok[k] && !fits55(vi[k])) {   // rare: exact value straight to the table
-              uint64_t* e = hot_entry(P, A, H, gid[k]);
-              if (e) { atomic_add_i128(e + 2 + A.key_words + d.word, vi[k]); if (d.track_seen) atomicOr(reinterpret_cast<unsigned long long*>(e + 1), 1ull << j); }
-              ok[k] = false;
-            }
-          }
+          av[k].i = 0; av[k].f = 0.0; av[k].valid = false;
+          if (gid[k] >= 0) av[k] = load_acc_value(d, c, threadIdx.x + k * NT);
         }
-        for (int g = 0; g < hot_n; ++g) {
-          uint64_t* wa = H.wacc + ((size_t)(warp * H.G + g)) * H.aw;
-          uint64_t* slot = wa + 1 + 2 * j;
-          bool any = false;
-#pragma unroll
-          for (int k = 0; k < RPT; ++k) any |= ok[k] && gid[k] == g;
-          const unsigned members = __ballot_sync(0xFFFFFFFFu, any);
-          if (members == 0) continue;
-          switch (d.op) {
-            case ACC_COUNT: {
-              int cnt = 0;
-#pragma unroll
-              for (int k = 0; k < RPT; ++k) cnt += (ok[k] && gid[k] == g) ? 1 : 0;
-              cnt = __reduce_add_sync(0xFFFFFFFFu, cnt);
-              if (lane == 0) slot[0] += (uint64_t)cnt;
-              break;
-            }
-            case ACC_SUM_I64: case ACC_SUM_I128: {
-              int64_t part = 0;
-#pragma unroll
-              for (int k = 0; k < RPT; ++k) part += (ok[k] && gid[k] == g) ? (int64_t)vi[k] : 0;
-              part = warp_sum_i64(part);
-              if (lane == 0) {
-                if (d.op == ACC_SUM_I64) slot[0] += (uint64_t)part;
-                else { const uint64_t lo = slot[0] + (uint64_t)part; slot[1] += (uint64_t)(part >> 63) + (lo < slot[0] ? 1ull : 0ull); slot[0] = lo; }
-              }
-              break;
-            }
-            case ACC_SUM_F64: {
-              double part = 0.0;
-#pragma unroll
-              for (int k = 0; k < RPT; ++k) part += (ok[k] && gid[k] == g) ? vf[k] : 0.0;
-              part = warp_sum_f64(part);
-              if (lane == 0) slot[0] = (uint64_t)__double_as_longlong(__longlong_as_double((long long)slot[0]) + part);
-              break;
-            }
-            default: {   // min / max (rarely hot) and the double-double sums: per thread, then a shuffle tree, then lane 0
-              uint64_t w0 = acc_identity(d.op, 0), w1 = acc_identity(d.op, 1);
-#pragma unroll
-              for (int k = 0; k < RPT; ++k) {
-                if (ok[k] && gid[k] == g) {
-                  const bool isf = d.op == ACC_MIN_F64 || d.op == ACC_MAX_F64 || acc_is_dd(d.op);
-                  const uint64_t v0 = isf ? (uint64_t)__double_as_longlong(vf[k]) : (uint64_t)(u128)vi[k];
-                  const uint64_t v1 = acc_is_dd(d.op) ? (uint64_t)(u128)vi[k] : isf ? 0 : (uint64_t)((u128)vi[k] >> 64);
-                  acc_combine_words(d.op, w0, w1, v0, v1);
-                }
-              }
-#pragma unroll
-              for (int dlt = 16; dlt; dlt >>= 1) {
-                const uint64_t o0 = __shfl_xor_sync(0xFFFFFFFFu, w0, dlt), o1 = __shfl_xor_sync(0xFFFFFFFFu, w1, dlt);
-                acc_combine_words(d.op, w0, w1, o0, o1);
-              }
-              if (lane == 0) { uint64_t a0 = slot[0], a1 = slot[1]; acc_combine_words(d.op, a0, a1, w0, w1); slot[0] = a0; slot[1] = a1; }
-            }
-          }
-          if (d.track_seen && lane == 0) wa[0] |= 1ull << j;
-        }
+        hot_fold<RPT>(H, A.hot_groups, A.n_accs, hot_n, A.key_words, d.op, d.word, j, d.track_seen != 0, av, gid,
+                      [&](int g) { return hot_entry(P, A, H, g); });
       }
     }
   }
@@ -1184,136 +1039,39 @@ __device__ __forceinline__ void sink_agg(const PipelineParams& P, const AggParam
   }
 }
 
-// ---- integer fast path: register-resident partials -------------------------------------------------
-// racc[g][j]: this thread's running 64-bit partial of accumulator j for hot group g.  Values are
-// admitted only below 2^55 in magnitude and the partials are spilled to the CTA accumulators (shared
-// memory atomics, once per REG_FLUSH rows) so they can never overflow.
-constexpr int REG_FLUSH = 224;    // 224 + RPT values below 2^55 cannot overflow 64 bits
-struct RegAcc { int64_t v[REG_GROUPS][REG_ACCS]; int rows; };
-
-__device__ __forceinline__ void reg_flush(const AggParams& A, const HotView& H, RegAcc& R, int hot_n) {
-  // CTA accumulators live in warp 0's wacc blocks: slot (g, j) = {lo, hi}.  The 32 lanes of a warp are summed with
-  // shuffles first, so only one lane per warp touches the shared accumulators (8-way instead of 256-way contention).
-  const int lane = threadIdx.x & 31;
-#pragma unroll
-  for (int g = 0; g < REG_GROUPS; ++g) {
-    if (g < hot_n) {
-      uint64_t* wa = H.wacc + (size_t)g * H.aw;
-#pragma unroll
-      for (int j = 0; j < REG_ACCS; ++j) {
-        if (j < A.n_accs) {
-          // |partial| < 2^63 per lane and the warp total may exceed 64 bits: reduce as 128-bit (lo, carry-aware hi)
-          const int64_t part = R.v[g][j];
-          unsigned long long lo = (unsigned long long)part;
-          long long hi = part >> 63;
-#pragma unroll
-          for (int d = 16; d; d >>= 1) {
-            const unsigned long long olo = __shfl_xor_sync(0xFFFFFFFFu, lo, d);
-            const long long ohi = __shfl_xor_sync(0xFFFFFFFFu, hi, d);
-            const unsigned long long s = lo + olo;
-            hi += ohi + (s < lo ? 1 : 0);
-            lo = s;
-          }
-          if (lane == 0 && (lo | (unsigned long long)hi)) {
-            unsigned long long* dst = reinterpret_cast<unsigned long long*>(wa + 1 + 2 * j);
-            const unsigned long long old = atomicAdd(dst, lo);
-            const unsigned long long carry = (old + lo) < old ? 1ull : 0ull;
-            const unsigned long long h2 = (unsigned long long)hi + carry;
-            if (h2) atomicAdd(dst + 1, h2);
-          }
-          R.v[g][j] = 0;
-        }
-      }
-    }
-  }
-  R.rows = 0;
-}
-
-// register path key handling: every key word is a plain 8-byte load (views, int64, decimals) unless the plan has
-// narrow or nullable keys, in which case the general packer runs; fingerprints are 32 bits so that the four
-// dictionary fingerprints arrive in one LDS.128
-__device__ __forceinline__ uint32_t reg_pack(const AggParams& A, const TileCtx& c, int r, uint64_t (&kw)[HOT_KEY_WORDS]) {
-  if (A.kw_simple) {
-#pragma unroll
-    for (int w = 0; w < HOT_KEY_WORDS; ++w)
-      kw[w] = w < A.key_words ? lds<uint64_t>(c.arena + A.kwords[w].slot + r * A.kwords[w].stride + A.kwords[w].byte_off) : 0ull;
-  } else {
-    pack_words(A, c, r, kw);
-  }
-  uint32_t fp = fold32(kw[0]);
-  fp = __funnelshift_l(fp, fp, 7) ^ fold32(kw[1]);
-  fp = __funnelshift_l(fp, fp, 7) ^ fold32(kw[2]);
-  fp = __funnelshift_l(fp, fp, 7) ^ fold32(kw[3]);
-  return fp;
-}
-__device__ __forceinline__ bool reg_verify(const HotView& H, int g, const uint64_t (&kw)[HOT_KEY_WORDS]) {
-  const ulonglong2* hk = reinterpret_cast<const ulonglong2*>(H.keys + g * HOT_KEY_WORDS);
-  const ulonglong2 a = hk[0], b = hk[1];
-  return a.x == kw[0] && a.y == kw[1] && b.x == kw[2] && b.y == kw[3];
-}
-__device__ __forceinline__ int reg_lookup(const HotView& H, int hot_n, const uint4& f4, const uint64_t (&kw)[HOT_KEY_WORDS], uint32_t fp) {
-  if (hot_n > 0 && f4.x == fp && reg_verify(H, 0, kw)) return 0;
-  if (hot_n > 1 && f4.y == fp && reg_verify(H, 1, kw)) return 1;
-  if (hot_n > 2 && f4.z == fp && reg_verify(H, 2, kw)) return 2;
-  if (hot_n > 3 && f4.w == fp && reg_verify(H, 3, kw)) return 3;
-  return -1;
-}
-
+// ---- integer fast path: register-resident partials (agg_hot.cuh: RegAcc) ------------------------------------------------
+// R.v[g][j]: this thread's running 64-bit partial of accumulator j for hot group g.
 template <int RPT>
-__device__ __forceinline__ void sink_agg_reg(const PipelineParams& P, const AggParams& A, const TileCtx& c, Smem* sm, RegAcc& R) {
+__device__ __forceinline__ void sink_agg_reg(const PipelineParams& P, const AggParams& A, const TileCtx& c, Smem* sm, RegAcc<REG_ACCS>& R) {
   const uint8_t* pact = P.mask_slot == NO_SLOT ? nullptr : c.arena + P.mask_slot;
-  HotView H = hot_view(A, c.arena);
+  const HotDict H = hot_dict(A, c.arena);
   int gid[RPT];
+  uint32_t fpv[RPT];
   bool live[RPT];
   bool miss = false;
-  const int hot_n0 = sm->hot_n;
-  const uint4 f4 = *reinterpret_cast<const uint4*>(H.fp32);
+  const int n0 = __shfl_sync(0xFFFFFFFFu, (int)lds_acquire_u32(&sm->dict_n), 0);      // warp-uniform (see sink_agg)
 #pragma unroll
   for (int k = 0; k < RPT; ++k) {
     const int r = threadIdx.x + k * NT;
     live[k] = r < c.nrows && (pact == nullptr || pact[r]);
-    gid[k] = -1;
+    gid[k] = -1; fpv[k] = 0;
     if (live[k]) {
-      uint64_t kw[HOT_KEY_WORDS];
-      const uint32_t fp = reg_pack(A, c, r, kw);
-      gid[k] = reg_lookup(H, hot_n0, f4, kw, fp);
+      HotKey kw;
+      reg_pack(A, c, r, kw);
+      fpv[k] = hot_fp(kw);
+      gid[k] = hot_lookup<REG_GROUPS>(H, n0, kw, fpv[k]);
       miss |= gid[k] < 0;
     }
   }
-  // dictionary growth (only while fewer than REG_GROUPS groups are known): same protocol as sink_agg
-  if (hot_n0 < REG_GROUPS) {
-    while (__syncthreads_or(miss && sm->hot_n < REG_GROUPS)) {
-      if (threadIdx.x == 0) sm->elect = NT;
-      __syncthreads();
-      const bool want = miss && sm->hot_n < REG_GROUPS;
-      if (want) atomicMin(&sm->elect, (int)threadIdx.x);
-      __syncthreads();
-      if (want && sm->elect == (int)threadIdx.x) {
-        for (int k = 0; k < RPT; ++k) {
-          if (live[k] && gid[k] < 0) {
-            uint64_t kw[HOT_KEY_WORDS];
-            const uint32_t fp = reg_pack(A, c, threadIdx.x + k * NT, kw);
-            const int g = sm->hot_n;
-            for (int w = 0; w < HOT_KEY_WORDS; ++w) H.keys[g * HOT_KEY_WORDS + w] = kw[w];
-            H.fp32[g] = fp;
-            H.entry[g] = 0;
-            sm->hot_n = g + 1;
-            break;
-          }
-        }
-      }
-      __syncthreads();
-      miss = false;
-      const int hot_n1 = sm->hot_n;
+  if (n0 < REG_GROUPS && __any_sync(0xFFFFFFFFu, miss)) {
 #pragma unroll
-      for (int k = 0; k < RPT; ++k) {
-        if (live[k] && gid[k] < 0) {
-          uint64_t kw[HOT_KEY_WORDS];
-          const uint32_t fp = reg_pack(A, c, threadIdx.x + k * NT, kw);
-          const uint4 g4 = *reinterpret_cast<const uint4*>(H.fp32);
-          gid[k] = reg_lookup(H, hot_n1, g4, kw, fp);
-          miss |= gid[k] < 0;
-        }
+    for (int k = 0; k < RPT; ++k) {
+      const bool want = live[k] && gid[k] < 0;
+      if (__any_sync(0xFFFFFFFFu, want)) {
+        HotKey kw;
+        reg_pack(A, c, threadIdx.x + k * NT, kw);
+        const int g = hot_dict_add<REG_GROUPS>(H, &sm->dict_n, &sm->dict_lock, REG_GROUPS, want, kw, fpv[k]);
+        if (want) gid[k] = g;
       }
     }
   }
@@ -1338,12 +1096,8 @@ __device__ __forceinline__ void sink_agg_reg(const PipelineParams& P, const AggP
             if (fits55(x)) val[j] = (int64_t)x;
             else {                                            // rare: exact value straight to the table entry
               uint64_t* e = hot_entry(P, A, H, gid[k]);
-              if (e) {
-                uint64_t* dst = e + 2 + A.key_words + A.accs[j].word;
-                // an Int64 sum has one word and is defined mod 2^64: no carry into the next accumulator
-                if (A.accs[j].op == ACC_SUM_I64) atomicAdd(reinterpret_cast<unsigned long long*>(dst), (unsigned long long)(int64_t)x);
-                else atomic_add_i128(dst, x);
-              }
+              // (an Int64 sum has one word and is defined mod 2^64: no carry into the next accumulator)
+              if (e) acc_apply(A.accs[j].op, e + 2 + A.key_words + A.accs[j].word, i128_lo(x), i128_hi(x));
             }
           }
         }
@@ -1368,65 +1122,12 @@ __device__ __forceinline__ void sink_agg_reg(const PipelineParams& P, const AggP
     }
   }
   R.rows += RPT;
-  if (R.rows >= REG_FLUSH) reg_flush(A, H, R, sm->hot_n);
+  if (R.rows >= REG_FLUSH) reg_flush(H, A.n_accs, R);
   {
     bool anycold = false;
 #pragma unroll
     for (int k = 0; k < RPT; ++k) anycold |= live[k] && gid[k] < 0;
     if (__any_sync(0xFFFFFFFFu, anycold)) agg_cold_rows<RPT>(P, A, c, gid, live);   // warp-level: no CTA barrier
-  }
-}
-
-__device__ __forceinline__ void hot_init(const AggParams& A, uint8_t* arena) {
-  if (A.hot_groups <= 0) return;
-  HotView H = hot_view(A, arena);
-  for (int i = threadIdx.x; i < NWARPS * H.G; i += NT) {
-    uint64_t* wa = H.wacc + (size_t)i * H.aw;
-    wa[0] = 0;
-    for (int j = 0; j < A.n_accs; ++j) { wa[1 + 2 * j] = acc_identity(A.accs[j].op, 0); wa[2 + 2 * j] = acc_identity(A.accs[j].op, 1); }
-  }
-}
-
-// end of kernel: fold the per-warp accumulators of every hot group into the global table
-__device__ __forceinline__ void hot_flush(const PipelineParams& P, const AggParams& A, uint8_t* arena, Smem* sm) {
-  if (A.hot_groups <= 0) return;
-  __syncthreads();
-  HotView H = hot_view(A, arena);
-  const int n = sm->hot_n;
-  for (int g = threadIdx.x; g < n; g += NT) hot_entry(P, A, H, g);
-  __syncthreads();
-  const int per = A.n_accs + 1;   // accumulators + the seen word
-  for (int p = threadIdx.x; p < n * per; p += NT) {
-    const int g = p / per, j = p % per;
-    uint64_t* e = reinterpret_cast<uint64_t*>(H.entry[g]);
-    if (!e) continue;
-    if (j == A.n_accs) {
-      uint64_t seen = 0;
-      for (int w = 0; w < NWARPS; ++w) seen |= H.wacc[((size_t)(w * H.G + g)) * H.aw];
-      if (seen) atomicOr(reinterpret_cast<unsigned long long*>(e + 1), (unsigned long long)seen);
-      continue;
-    }
-    const AccDesc& d = A.accs[j];
-    uint64_t w0 = acc_identity(d.op, 0), w1 = acc_identity(d.op, 1);
-    if (d.op == ACC_SUM_I128) { w0 = 0; w1 = 0; }
-    for (int w = 0; w < NWARPS; ++w) {
-      const uint64_t* slot = H.wacc + ((size_t)(w * H.G + g)) * H.aw + 1 + 2 * j;
-      acc_combine_words(d.op, w0, w1, slot[0], slot[1]);
-    }
-    uint64_t* dst = e + 2 + A.key_words + d.word;
-    switch (d.op) {
-      case ACC_SUM_I64: case ACC_COUNT: if (w0) atomicAdd(reinterpret_cast<unsigned long long*>(dst), (unsigned long long)w0); break;
-      case ACC_SUM_I128: atomic_add_i128(dst, (i128)(((u128)w1 << 64) | w0)); break;
-      case ACC_SUM_F64: atomicAdd(reinterpret_cast<double*>(dst), __longlong_as_double((long long)w0)); break;
-      case ACC_MIN_I32: case ACC_MIN_I64: atomicMin(reinterpret_cast<long long*>(dst), (long long)w0); break;
-      case ACC_MAX_I32: case ACC_MAX_I64: atomicMax(reinterpret_cast<long long*>(dst), (long long)w0); break;
-      case ACC_MIN_I128: atomic_minmax_i128(dst, (i128)(((u128)w1 << 64) | w0), true); break;
-      case ACC_MAX_I128: atomic_minmax_i128(dst, (i128)(((u128)w1 << 64) | w0), false); break;
-      case ACC_MIN_F64: atomic_minmax_f64(dst, __longlong_as_double((long long)w0), true); break;
-      case ACC_MAX_F64: atomic_minmax_f64(dst, __longlong_as_double((long long)w0), false); break;
-      case ACC_DD_SUM: case ACC_DD_SQ: atomic_add_dd(dst, __longlong_as_double((long long)w0), __longlong_as_double((long long)w1)); break;
-      default: break;
-    }
   }
 }
 
@@ -1816,11 +1517,14 @@ __global__ void __launch_bounds__(NT, MINB) pipeline_kernel(const __grid_constan
     mbar_init(&sm->full[0], 1);
     mbar_init(&sm->full[1], 1);
     fence_barrier_init();
-    sm->hot_n = 0;
+    sm->dict_n = 0; sm->dict_lock = 0;
     sm->tile[0] = dynamic ? (int)atomicAdd(P0.ticket, 1u) : (int)blockIdx.x;
     sm->defer[0] = guarded ? table_full() : 0;
   }
-  if (KC == KC_AGG) hot_init(K.aux[0].agg, arena);
+  if (KC == KC_AGG && K.aux[0].agg.hot_groups > 0) {
+    const AggParams& A = K.aux[0].agg;
+    hot_init(hot_dict(A, arena), A.hot_groups, A.n_accs, [&](int j) { return (int)A.accs[j].op; });
+  }
   if (KC == KC_OTHER && P0.sink == SINK_BUILD) {
     unsigned long long* z = reinterpret_cast<unsigned long long*>(arena + K.aux[0].build.smem_off);
     for (int i = threadIdx.x; i < CHAIN_CACHE_ENTRIES * 3; i += NT) z[i] = 0ull;
@@ -1854,7 +1558,7 @@ __global__ void __launch_bounds__(NT, MINB) pipeline_kernel(const __grid_constan
     return true;
   };
 
-  RegAcc R;
+  RegAcc<REG_ACCS> R;
 #pragma unroll
   for (int g = 0; g < REG_GROUPS; ++g)
 #pragma unroll
@@ -1925,9 +1629,12 @@ __global__ void __launch_bounds__(NT, MINB) pipeline_kernel(const __grid_constan
   }
   if (KC == KC_OTHER && P0.sink == SINK_BUILD)
     chain_cache_flush(K.aux[0].build, reinterpret_cast<ChainCacheEntry*>(arena + K.aux[0].build.smem_off), &sm->cache_count);
-  if constexpr (KC == KC_AGG) {
-    if (K.aux[0].agg.reg_path) { HotView H = hot_view(K.aux[0].agg, arena); reg_flush(K.aux[0].agg, H, R, sm->hot_n); }
-    hot_flush(P0, K.aux[0].agg, arena, sm);
+  if (KC == KC_AGG && K.aux[0].agg.hot_groups > 0) {
+    const AggParams& A = K.aux[0].agg;
+    const HotDict H = hot_dict(A, arena);
+    if (A.reg_path) reg_flush(H, A.n_accs, R);
+    hot_flush(H, &sm->dict_n, A.hot_groups, A.n_accs, A.key_words, [&](int j) { return (int)A.accs[j].op; }, [&](int j) { return (int)A.accs[j].word; },
+              [&](int g) { return hot_entry(P0, A, H, g); });
   }
 }
 

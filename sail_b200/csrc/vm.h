@@ -28,7 +28,14 @@ constexpr int MAX_DISTINCT = 4;    // pair sets (distinct arguments) of one aggr
 constexpr int REG_GROUPS = 4;      // hot groups held in registers by the integer fast path
 constexpr int REG_ACCS = 6;        // accumulators held in registers per group
 constexpr int HOT_KEY_WORDS = 4;   // group keys wider than 32 bytes skip the hot paths (global table only)
+constexpr int HOT_MAX_GROUPS = 8;  // groups of the CTA dictionary (agg_hot.cuh): eight fingerprints in two LDS.128
 constexpr uint32_t NO_SLOT = 0xFFFFFFFFu;
+
+// shared-memory bytes of a CTA dictionary of `groups` hot groups (agg_hot.cuh): fingerprints, keys, entry pointers and one
+// accumulator block per warp and group
+__host__ __device__ constexpr uint32_t hot_scratch_bytes(int groups, int n_accs) {
+  return groups <= 0 ? 0u : (uint32_t)(32 + groups * (HOT_KEY_WORDS * 8 + 8) + (NT / 32) * groups * (1 + 2 * n_accs) * 8 + 127) & ~127u;
+}
 
 enum VmKind : uint8_t { K_B = 0, K_I32 = 1, K_I64 = 2, K_F64 = 3, K_I128 = 4, K_V16 = 5 };
 __host__ __device__ inline int kind_width(int k) { return k == K_B ? 1 : k == K_I32 ? 4 : (k == K_I64 || k == K_F64) ? 8 : 16; }
