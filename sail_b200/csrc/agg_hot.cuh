@@ -1,5 +1,5 @@
-// agg_hot.cuh -- the CTA dictionary of hot groups and the accumulator updates of a hash aggregate, shared by the interpreted
-// kernel (pipeline.cu) and the specialised kernels (jit_rt.cuh).
+// agg_hot.cuh -- the global group table, the CTA dictionary of hot groups and the accumulator updates of a hash aggregate,
+// shared by the interpreted kernel (pipeline.cu) and the specialised kernels (jit_rt.cuh).
 //
 // Low-cardinality grouping (TPC-H Q1: 4 groups) keeps the first groups a CTA sees in a dictionary in shared memory, laid out
 // as hot_scratch_bytes (vm.h) counts it:
@@ -10,8 +10,9 @@
 // Entries are immutable once published; dict_n is released after the entry is written, so readers need no lock.  Growth
 // takes a CTA-wide spin lock, one lane per warp at a time, so no warp waits on a CTA barrier for it.
 //
-// The functions take the accumulator's operator, word and counts as plain arguments: the interpreter passes its AggParams,
-// the specialised kernel the constants of its G, which fold away once inlined.
+// The functions take the accumulator's operator, word and counts as plain arguments, and small lambdas for what the kernels
+// do differently (key packing, hashing and comparison): the interpreter passes its AggParams, the specialised kernel the
+// constants of its G, which fold away once inlined.
 #pragma once
 #include "dev_ops.cuh"
 
@@ -74,6 +75,92 @@ __device__ __forceinline__ void acc_global(uint64_t* e, int key_words, int op, i
   acc_val_words(op, v, w0, w1);
   acc_apply(op, dst, w0, w1);
   if (seen) acc_mark_seen(e, j);
+}
+
+// ---- the global group table --------------------------------------------------------------------
+constexpr int FROM_A = -1;
+// Entry of EW words: [hash][seen bits][KW key words][accumulators], probed linearly from hash & capacity_mask.  EW and KW are
+// the specialised kernel's constants; FROM_A reads A.entry_words / A.key_words where they are used, which costs the
+// interpreter fewer registers than values held across the probe loop.
+// State word: 0 = empty, else (tag30 << 2) | {1 = being written, 2 = ready}.  Carrying the tag in the state lets a thread skip
+// a slot that is being written for a different key without waiting on it.
+// init(A, acc) writes the accumulator identities of a fresh entry (acc: its first accumulator word); eq(A, k, key) compares the
+// key words k of an entry with `key`.  They take A as an argument rather than capturing it: a capture costs the interpreter
+// registers.  `claimed` (optional) is set when this call inserted the key: exactly one caller per key sees it.
+template <int EW, int KW, class Key, class Init, class Eq>
+__device__ __forceinline__ uint64_t* find_or_insert(const AggParams& A, const Key& key, uint64_t h, uint32_t* err, Init init, Eq eq,
+                                                    bool* claimed = nullptr) {
+  const uint32_t tag = (uint32_t)(h >> 34) << 2;
+  uint64_t idx = h & A.capacity_mask;
+  uint64_t probes = 0;
+  uint32_t spins = 0;
+  while (probes <= A.capacity_mask) {
+    uint64_t* e = reinterpret_cast<uint64_t*>(A.table) + idx * (EW != FROM_A ? (uint32_t)EW : A.entry_words);
+    uint32_t* st = A.state + idx;
+    uint32_t s = ld_acquire_u32(st);
+    if (s == ST_EMPTY) {
+      s = atomicCAS(st, ST_EMPTY, tag | ST_LOCKED);
+      if (s == ST_EMPTY) {
+        e[0] = h;
+        e[1] = 0;                                                   // seen
+        if constexpr (KW != FROM_A) {
+#pragma unroll
+          for (int w = 0; w < KW; ++w) e[2 + w] = key.w[w];
+        } else {
+          for (int w = 0; w < A.key_words; ++w) e[2 + w] = key.w[w];
+        }
+        init(A, e + 2 + (KW != FROM_A ? KW : A.key_words));
+        st_release_u32(st, tag | ST_READY);                         // release: the entry words above are visible first
+        if (claimed) *claimed = true;
+        {
+          // occupied-slot list: one counter for the whole table, so the increment is aggregated over the lanes
+          // that insert in the same step (same-address atomics serialise in one L2 slice)
+          const unsigned m = __activemask();
+          const unsigned lane = threadIdx.x & 31;
+          const int lead = __ffs(m) - 1;
+          unsigned long long base = 0;
+          if ((int)lane == lead) base = atomicAdd(A.n_groups, (unsigned long long)__popc(m));
+          base = __shfl_sync(m, base, lead);
+          A.occ[base + __popc(m & ((1u << lane) - 1))] = (uint32_t)idx;
+        }
+        return e;
+      }
+    }
+    if ((s & ~3u) == tag) {
+      if ((s & 3u) == ST_LOCKED) {          // same tag, still being published: look again (bounded)
+        if (++spins > (1u << 24)) { atomicOr(err, ERR_TABLE_FULL); return nullptr; }
+        __nanosleep(32);
+        continue;
+      }
+      if (e[0] == h && eq(A, e + 2, key)) return e;
+    }
+    idx = (idx + 1) & A.capacity_mask;
+    ++probes;
+  }
+  atomicOr(err, ERR_TABLE_FULL);
+  return nullptr;
+}
+
+// Warp-cooperative front end: lanes of one warp that carry the same key hash elect a leader (__match_any_sync); only leaders
+// touch the table, followers receive the entry pointer by shuffle.  Removes same-warp contention on a slot that is being
+// published.  All 32 lanes must call; lanes without `need` get nullptr.
+// `claimed` (optional): this lane's key was inserted by this call -- by the lane itself, never for a follower.
+template <int EW, int KW, class Key, class Init, class Eq>
+__device__ __forceinline__ uint64_t* find_or_insert_warp(const AggParams& A, const Key& key, uint64_t h, bool need, uint32_t* err,
+                                                         Init init, Eq eq, bool* claimed = nullptr) {
+  const unsigned lane = threadIdx.x & 31;
+  const unsigned long long probe = need ? h : (0xFFFFFFFF00000000ull | lane);   // idle lanes match nobody useful
+  const unsigned peers = __match_any_sync(0xFFFFFFFFu, probe);
+  const int leader = __ffs(peers) - 1;
+  uint64_t* e = nullptr;
+  bool mine = false;
+  if (need && (int)lane == leader) e = find_or_insert<EW, KW>(A, key, h, err, init, eq, &mine);
+  unsigned long long p = __shfl_sync(0xFFFFFFFFu, reinterpret_cast<unsigned long long>(e), leader);
+  uint64_t* got = reinterpret_cast<uint64_t*>(p);
+  // same hash but different key (64-bit collision inside one warp): fall back to an own lookup
+  if (need && (int)lane != leader && got && !eq(A, got + 2, key)) got = find_or_insert<EW, KW>(A, key, h, err, init, eq, &mine);
+  if (claimed) *claimed = mine;
+  return need ? got : nullptr;
 }
 
 // ---- the dictionary ----------------------------------------------------------------------------
@@ -161,6 +248,56 @@ __device__ __noinline__ int hot_dict_add(const HotDict H, uint32_t* dict_n, uint
   return g;
 }
 
+// Warp-collective: gid[k] of every live row k is its group in the dictionary -- appended while the dictionary holds fewer than
+// cap (<= CAP) groups -- or -1.  pack(k, kw) packs row k's key.
+template <int CAP, int RPT, class Pack>
+__device__ __forceinline__ void hot_assign(const HotDict& H, uint32_t* dict_n, uint32_t* dict_lock, int cap, const bool (&live)[RPT],
+                                           int (&gid)[RPT], Pack pack) {
+  uint32_t fpv[RPT];
+  bool miss = false;
+  // The lanes of a warp arrive one by one and other warps grow the dictionary meanwhile: lanes that read different sizes
+  // would split around the warp collectives below and hang the warp.  Lane 0's reading is broadcast, so that those
+  // collectives are executed by all lanes or by none.
+  const int n0 = __shfl_sync(0xFFFFFFFFu, (int)lds_acquire_u32(dict_n), 0);
+#pragma unroll
+  for (int k = 0; k < RPT; ++k) {
+    gid[k] = -1; fpv[k] = 0;
+    if (live[k]) {
+      HotKey kw;
+      pack(k, kw);
+      fpv[k] = hot_fp(kw);
+      gid[k] = hot_lookup<CAP>(H, n0, kw, fpv[k]);
+      miss |= gid[k] < 0;
+    }
+  }
+  if (n0 < cap && __any_sync(0xFFFFFFFFu, miss)) {
+#pragma unroll
+    for (int k = 0; k < RPT; ++k) {
+      const bool want = live[k] && gid[k] < 0;
+      if (__any_sync(0xFFFFFFFFu, want)) {
+        HotKey kw;
+        pack(k, kw);
+        const int g = hot_dict_add<CAP>(H, dict_n, dict_lock, cap, want, kw, fpv[k]);
+        if (want) gid[k] = g;
+      }
+    }
+  }
+}
+
+// The table entry of dictionary group g, inserted from the dictionary's copy of the key (hashed with hash(A, key)) on first use.
+// Other warps store the same pointer meanwhile (a benign race), hence the volatile load.
+template <int EW, int KW, class Key, class Hash, class Init, class Eq>
+__device__ __noinline__ uint64_t* hot_entry(const HotDict H, int g, const AggParams& A, uint32_t* err, Hash hash, Init init, Eq eq) {
+  uint64_t* e = reinterpret_cast<uint64_t*>(*reinterpret_cast<volatile uint64_t*>(H.entry + g));
+  if (e) return e;
+  Key key;
+#pragma unroll
+  for (int w = 0; w < (int)(sizeof(Key) / 8); ++w) key.w[w] = (w < (KW != FROM_A ? KW : A.key_words) && w < HOT_KEY_WORDS) ? H.keys[g * HOT_KEY_WORDS + w] : 0ull;
+  e = find_or_insert<EW, KW>(A, key, hash(A, key), err, init, eq);
+  H.entry[g] = reinterpret_cast<uint64_t>(e);
+  return e;
+}
+
 // ---- per-warp accumulator blocks ---------------------------------------------------------------
 template <class OpOf>
 __device__ __forceinline__ void hot_init(const HotDict& H, int groups, int n_accs, OpOf op_of) {
@@ -242,6 +379,29 @@ __device__ __forceinline__ void hot_fold(const HotDict& H, int groups, int n_acc
 // so they never overflow.
 constexpr int REG_FLUSH = 224;    // 224 + RPT values below 2^55 cannot overflow 64 bits
 template <int NA> struct RegAcc { int64_t v[REG_GROUPS][NA]; int rows; };
+
+// one row's values into the partials of its group g (0 <= g < REG_GROUPS)
+template <int NA>
+__device__ __forceinline__ void reg_add(RegAcc<NA>& R, int g, const int64_t (&val)[NA]) {
+  static_assert(REG_GROUPS == 4, "one case per register group");
+  switch (g) {            // only this row's group is touched (divergent, but 4x fewer adds than predication)
+    case 0:
+#pragma unroll
+      for (int j = 0; j < NA; ++j) R.v[0][j] += val[j];
+      break;
+    case 1:
+#pragma unroll
+      for (int j = 0; j < NA; ++j) R.v[1][j] += val[j];
+      break;
+    case 2:
+#pragma unroll
+      for (int j = 0; j < NA; ++j) R.v[2][j] += val[j];
+      break;
+    default:
+#pragma unroll
+      for (int j = 0; j < NA; ++j) R.v[3][j] += val[j];
+  }
+}
 
 // Warp-collective (full-mask shuffles): nothing in here may depend on the dictionary size, which other warps change
 // asynchronously -- every register group is flushed, groups that do not exist yet hold zeros.  The 32 lanes are summed with

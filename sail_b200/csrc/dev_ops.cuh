@@ -1,6 +1,6 @@
 // dev_ops.cuh -- small device helpers shared by the interpreter kernel (pipeline.cu) and the runtime of the
 // specialised (NVRTC-compiled) pipeline kernels (jit_rt.cuh): wrapping arithmetic, date/LIKE helpers, accumulator
-// identities and combiners, 128-bit atomics.
+// identities and combiners, 128-bit atomics, the ordered compaction of a tile.
 #pragma once
 #include "dev_util.cuh"
 #include "vm.h"
@@ -373,6 +373,71 @@ __device__ __forceinline__ int32_t view_char_length(const ulonglong2& v) {
   if (p + 2 <= e) { c += utf8_cont_bytes(__ldg(reinterpret_cast<const unsigned short*>(p))); p += 2; }
   if (p < e) c += utf8_cont_bytes(__ldg(p));
   return (int32_t)(n - c);
+}
+
+// Order-preserving compaction of tile `tile` (tile_rows rows; thread row k is threadIdx.x + k * NT, keep[k]: it is kept), called
+// by the whole CTA: returns the output position of the tile's first kept row, and at[k] = the position of kept row k within
+// the tile.  warp_sums (RPT * NT / 32 words) and tile_base are the CTA's shared scratch; the caller needs a CTA barrier before
+// they are written again.  The tile that ends the input writes P.out_count.
+// Look-back word of P.tile_status: bits 63..62 = 0 invalid / 1 tile aggregate / 2 inclusive prefix.
+template <int RPT>
+__device__ __forceinline__ unsigned long long compact_positions(const PipelineParams& P, const bool (&keep)[RPT], int64_t tile, int tile_rows,
+                                                                uint32_t* warp_sums, unsigned long long* tile_base, uint32_t (&at)[RPT]) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int k = 0; k < RPT; ++k) {
+    const uint32_t b = __ballot_sync(0xFFFFFFFFu, keep[k]);
+    at[k] = __popc(b & ((1u << lane) - 1));
+    if (lane == 0) warp_sums[k * (NT / 32) + warp] = __popc(b);
+  }
+  __syncthreads();
+  if (warp == 0) {
+    // exclusive scan of the RPT * 8 (<= 32) warp totals, in row order
+    const int n = RPT * (NT / 32);
+    uint32_t v = lane < n ? warp_sums[lane] : 0, incl = v;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) { uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, d); if (lane >= d) incl += t; }
+    if (lane < n) warp_sums[lane] = incl - v;
+    const uint32_t total = __shfl_sync(0xFFFFFFFFu, incl, 31);
+    // decoupled look-back, one warp wide: 32 predecessor tiles are inspected per step; the walk stops at the
+    // closest tile that already published an inclusive prefix (flag 2) and adds the aggregates (flag 1) in between
+    unsigned long long excl = 0;
+    if (P.tile_offsets) {
+      excl = P.tile_offsets[tile];             // two-pass filter: the mask pass already fixed every tile's position
+    } else if (tile > 0) {
+      if (lane == 0) st_release_u64(P.tile_status + tile, (1ull << 62) | total);
+      int64_t hi = tile - 1;                   // newest tile not yet accounted for
+      uint32_t spins = 0;
+      for (;;) {
+        const int64_t t = hi - lane;
+        unsigned long long sw = t >= 0 ? ld_acquire_u64(P.tile_status + t) : (2ull << 62);   // before tile 0: prefix 0
+        const unsigned flag = (unsigned)(sw >> 62);
+        const unsigned ready = __ballot_sync(0xFFFFFFFFu, flag != 0);
+        const unsigned prefix = __ballot_sync(0xFFFFFFFFu, flag == 2);
+        // usable window: lanes 0..first_prefix (inclusive) if all of them are ready
+        const int first_prefix = prefix ? __ffs(prefix) - 1 : 32;
+        const unsigned need = first_prefix >= 31 ? 0xFFFFFFFFu : ((2u << first_prefix) - 1);
+        if ((ready & need) != need) { if (++spins > (1u << 24)) __trap(); continue; }      // somebody in the window is not published yet
+        unsigned long long s = (lane <= first_prefix) ? (sw & ((1ull << 62) - 1)) : 0ull;
+#pragma unroll
+        for (int d = 16; d; d >>= 1) s += __shfl_xor_sync(0xFFFFFFFFu, s, d);
+        excl += s;
+        if (first_prefix < 32) break;          // reached a published prefix
+        hi -= 32;
+      }
+    }
+    if (lane == 0) {
+      *tile_base = excl;
+      if (!P.tile_offsets) {
+        st_release_u64(P.tile_status + tile, (2ull << 62) | (excl + total));
+        if ((tile + 1) * tile_rows >= P.n_rows) *P.out_count = excl + total;
+      }
+    }
+  }
+  __syncthreads();
+#pragma unroll
+  for (int k = 0; k < RPT; ++k) at[k] += warp_sums[k * (NT / 32) + warp];
+  return *tile_base;
 }
 
 }  // namespace sg

@@ -94,81 +94,29 @@ __device__ __noinline__ bool jit_like(ulonglong2 v, const uint8_t* pat, uint32_t
 }
 
 // ================================================================================================
-// global group table (layout and protocol of pipeline.cu::agg_find_or_insert, constants from G)
+// global group table (agg_hot.cuh), constants from G
 // ================================================================================================
+// G's arguments to the group-table functions: identities of its accumulators, its key comparison
 template <class G>
-__device__ __forceinline__ uint64_t* jit_find_or_insert(const AggParams& A, const typename G::Key& kw, uint64_t h, uint32_t* err) {
-  const uint32_t tag = (uint32_t)(h >> 34) << 2;
-  uint64_t idx = h & A.capacity_mask;
-  uint64_t probes = 0;
-  uint32_t spins = 0;
-  while (probes <= A.capacity_mask) {
-    uint64_t* e = reinterpret_cast<uint64_t*>(A.table) + idx * G::ENTRY_WORDS;
-    uint32_t* st = A.state + idx;
-    uint32_t s = ld_acquire_u32(st);
-    if (s == ST_EMPTY) {
-      s = atomicCAS(st, ST_EMPTY, tag | ST_LOCKED);
-      if (s == ST_EMPTY) {
-        e[0] = h;
-        e[1] = 0;
+__device__ __forceinline__ auto jit_init() {
+  return [](const AggParams&, uint64_t* acc) {
+    static_for<0, G::N_ACCS>([&](auto Jc) { constexpr int J = decltype(Jc)::value;
 #pragma unroll
-        for (int w = 0; w < G::KEY_WORDS; ++w) e[2 + w] = kw.w[w];
-        static_for<0, G::N_ACCS>([&](auto Jc) { constexpr int J = decltype(Jc)::value;
-#pragma unroll
-          for (int w = 0; w < acc_words_of(G::acc_op(J)); ++w) e[2 + G::KEY_WORDS + G::acc_word(J) + w] = acc_identity(G::acc_op(J), w);
-        });
-        st_release_u32(st, tag | ST_READY);
-        {
-          const unsigned m = __activemask();
-          const unsigned lane = threadIdx.x & 31;
-          const int lead = __ffs(m) - 1;
-          unsigned long long base = 0;
-          if ((int)lane == lead) base = atomicAdd(A.n_groups, (unsigned long long)__popc(m));
-          base = __shfl_sync(m, base, lead);
-          A.occ[base + __popc(m & ((1u << lane) - 1))] = (uint32_t)idx;
-        }
-        return e;
-      }
-    }
-    if ((s & ~3u) == tag) {
-      if ((s & 3u) == ST_LOCKED) {
-        if (++spins > (1u << 24)) { atomicOr(err, ERR_TABLE_FULL); return nullptr; }
-        __nanosleep(32);
-        continue;
-      }
-      if (e[0] == h && G::keys_equal(e + 2, kw)) return e;
-    }
-    idx = (idx + 1) & A.capacity_mask;
-    ++probes;
-  }
-  atomicOr(err, ERR_TABLE_FULL);
-  return nullptr;
+      for (int w = 0; w < acc_words_of(G::acc_op(J)); ++w) acc[G::acc_word(J) + w] = acc_identity(G::acc_op(J), w);
+    });
+  };
 }
-
 template <class G>
-__device__ __forceinline__ uint64_t* jit_find_or_insert_warp(const AggParams& A, const typename G::Key& kw, uint64_t h, bool need, uint32_t* err) {
-  const unsigned lane = threadIdx.x & 31;
-  const unsigned long long probe = need ? h : (0xFFFFFFFF00000000ull | lane);
-  const unsigned peers = __match_any_sync(0xFFFFFFFFu, probe);
-  const int leader = __ffs(peers) - 1;
-  uint64_t* e = nullptr;
-  if (need && (int)lane == leader) e = jit_find_or_insert<G>(A, kw, h, err);
-  unsigned long long p = __shfl_sync(0xFFFFFFFFu, reinterpret_cast<unsigned long long>(e), leader);
-  uint64_t* got = reinterpret_cast<uint64_t*>(p);
-  if (need && (int)lane != leader && got && !G::keys_equal(got + 2, kw)) got = jit_find_or_insert<G>(A, kw, h, err);
-  return need ? got : nullptr;
+__device__ __forceinline__ auto jit_eq() {
+  return [](const AggParams&, const uint64_t* k, const typename G::Key& key) { return G::keys_equal(k, key); };
 }
-
+// entry_of(g): the table entry of dictionary group g (agg_hot.cuh: hot_entry)
 template <class G>
-__device__ __noinline__ uint64_t* jit_hot_entry(const KernelArgs& K, const HotDict H, int g) {
-  uint64_t* e = reinterpret_cast<uint64_t*>(*reinterpret_cast<volatile uint64_t*>(H.entry + g));
-  if (e) return e;
-  typename G::Key kw;
-#pragma unroll
-  for (int w = 0; w < HOT_KEY_WORDS; ++w) kw.w[w] = w < G::KEY_WORDS ? H.keys[g * HOT_KEY_WORDS + w] : 0ull;
-  e = jit_find_or_insert<G>(K.aux[0].agg, kw, G::key_hash(kw), K.P[0].error_flag);
-  H.entry[g] = reinterpret_cast<uint64_t>(e);       // benign race: every writer stores the same pointer
-  return e;
+__device__ __forceinline__ auto jit_entry_of(const KernelArgs& K, const HotDict& H) {
+  return [&K, H](int g) {
+    return hot_entry<G::ENTRY_WORDS, G::KEY_WORDS, typename G::Key>(H, g, K.aux[0].agg, K.P[0].error_flag,
+                                                                      [](const AggParams&, const typename G::Key& k) { return G::key_hash(k); }, jit_init<G>(), jit_eq<G>());
+  };
 }
 
 // warp-level pre-aggregation of one accumulator (jit_cold_rows): `prepare` turns a row's value into a partial state (count(*) of
@@ -226,7 +174,7 @@ __device__ __forceinline__ void jit_cold_rows(const KernelArgs& K, const typenam
     if (__any_sync(0xFFFFFFFFu, cold)) {
       typename G::Key kw;
       G::key_words(rows[k], kw);
-      uint64_t* e = jit_find_or_insert_warp<G>(A, kw, hh[k], cold, K.P[0].error_flag);
+      uint64_t* e = find_or_insert_warp<G::ENTRY_WORDS, G::KEY_WORDS>(A, kw, hh[k], cold, K.P[0].error_flag, jit_init<G>(), jit_eq<G>());
       // Rows of one group that sit in the same warp (clustered inputs: the 1-7 lineitems of an order are neighbours) are combined
       // in registers first: one set of accumulator atomics per (warp, group) instead of per row.  The atomics are what bounds this
       // path -- every accumulator adds atomics on top of the inserts.
@@ -267,39 +215,15 @@ template <class G>
 __device__ __forceinline__ void jit_agg_reg_tile(const KernelArgs& K, const typename G::Row (&rows)[G::RPT], JitSmem* sm, uint8_t* scratch, JitAggRegs<G>& R) {
   static_assert(sizeof(typename G::Key) == sizeof(HotKey), "dictionary tiers hold keys of at most HOT_KEY_WORDS words");
   const HotDict H = hot_dict(scratch, G::HOT_G);
+  bool live[G::RPT];
+#pragma unroll
+  for (int k = 0; k < G::RPT; ++k) live[k] = rows[k].live;
   int gid[G::RPT];
-  uint32_t fpv[G::RPT];
-  bool miss = false;
-  // the lanes of a warp leave the mbarrier wait one by one and other warps grow the dictionary meanwhile: lane 0's reading is
-  // broadcast so that the warp collectives below are executed by all lanes or by none
-  const int n0 = __shfl_sync(0xFFFFFFFFu, (int)lds_acquire_u32(&sm->dict_n), 0);
-#pragma unroll
-  for (int k = 0; k < G::RPT; ++k) {
-    gid[k] = -1; fpv[k] = 0;
-    if (rows[k].live) {
-      typename G::Key kw;
-      G::key_words(rows[k], kw);
-      fpv[k] = hot_fp(kw);
-      gid[k] = hot_lookup<REG_GROUPS>(H, n0, kw, fpv[k]);
-      miss |= gid[k] < 0;
-    }
-  }
-  if (n0 < REG_GROUPS && __any_sync(0xFFFFFFFFu, miss)) {
-#pragma unroll
-    for (int k = 0; k < G::RPT; ++k) {
-      const bool want = rows[k].live && gid[k] < 0;
-      if (__any_sync(0xFFFFFFFFu, want)) {
-        typename G::Key kw;
-        G::key_words(rows[k], kw);
-        const int g = hot_dict_add<REG_GROUPS>(H, &sm->dict_n, &sm->dict_lock, REG_GROUPS, want, kw, fpv[k]);
-        if (want) gid[k] = g;
-      }
-    }
-  }
+  hot_assign<REG_GROUPS>(H, &sm->dict_n, &sm->dict_lock, REG_GROUPS, live, gid, [&](int k, HotKey& kw) { G::key_words(rows[k], kw); });
 #pragma unroll
   for (int k = 0; k < G::RPT; ++k) {
     if (rows[k].live && gid[k] >= 0) {
-      int64_t val[G::N_ACCS > 0 ? G::N_ACCS : 1];
+      int64_t val[G::N_ACCS > 0 ? G::N_ACCS : 1] = {};
       static_for<0, G::N_ACCS>([&](auto Jc) { constexpr int J = decltype(Jc)::value;
         constexpr int mode = G::reg_mode(J);
         if constexpr (mode == 0) val[J] = 1;
@@ -310,30 +234,14 @@ __device__ __forceinline__ void jit_agg_reg_tile(const KernelArgs& K, const type
             if (fits55(a.i)) val[J] = (int64_t)a.i;
             else {                                               // rare: exact value straight to the table entry
               val[J] = 0;
-              uint64_t* e = jit_hot_entry<G>(K, H, gid[k]);
+              uint64_t* e = jit_entry_of<G>(K, H)(gid[k]);
               // (an Int64 sum has one word and is defined mod 2^64: no carry into the next accumulator)
               if (e) acc_apply(G::acc_op(J), e + 2 + G::KEY_WORDS + G::acc_word(J), i128_lo(a.i), i128_hi(a.i));
             }
           }
         }
       });
-      switch (gid[k]) {
-        case 0:
-#pragma unroll
-          for (int j = 0; j < G::N_ACCS; ++j) R.v[0][j] += val[j];
-          break;
-        case 1:
-#pragma unroll
-          for (int j = 0; j < G::N_ACCS; ++j) R.v[1][j] += val[j];
-          break;
-        case 2:
-#pragma unroll
-          for (int j = 0; j < G::N_ACCS; ++j) R.v[2][j] += val[j];
-          break;
-        default:
-#pragma unroll
-          for (int j = 0; j < G::N_ACCS; ++j) R.v[3][j] += val[j];
-      }
+      reg_add(R, gid[k], val);
     }
   }
   R.rows += G::RPT;
@@ -349,33 +257,11 @@ template <class G>
 __device__ __forceinline__ void jit_agg_dict_tile(const KernelArgs& K, const typename G::Row (&rows)[G::RPT], JitSmem* sm, uint8_t* scratch) {
   static_assert(sizeof(typename G::Key) == sizeof(HotKey), "dictionary tiers hold keys of at most HOT_KEY_WORDS words");
   const HotDict H = hot_dict(scratch, G::HOT_G);
+  bool live[G::RPT];
+#pragma unroll
+  for (int k = 0; k < G::RPT; ++k) live[k] = rows[k].live;
   int gid[G::RPT];
-  uint32_t fpv[G::RPT];
-  bool miss = false;
-  const int n0 = __shfl_sync(0xFFFFFFFFu, (int)lds_acquire_u32(&sm->dict_n), 0);      // warp-uniform (see jit_agg_reg_tile)
-#pragma unroll
-  for (int k = 0; k < G::RPT; ++k) {
-    gid[k] = -1; fpv[k] = 0;
-    if (rows[k].live) {
-      typename G::Key kw;
-      G::key_words(rows[k], kw);
-      fpv[k] = hot_fp(kw);
-      gid[k] = hot_lookup<G::HOT_G>(H, n0, kw, fpv[k]);
-      miss |= gid[k] < 0;
-    }
-  }
-  if (n0 < G::HOT_G && __any_sync(0xFFFFFFFFu, miss)) {
-#pragma unroll
-    for (int k = 0; k < G::RPT; ++k) {
-      const bool want = rows[k].live && gid[k] < 0;
-      if (__any_sync(0xFFFFFFFFu, want)) {
-        typename G::Key kw;
-        G::key_words(rows[k], kw);
-        const int g = hot_dict_add<G::HOT_G>(H, &sm->dict_n, &sm->dict_lock, G::HOT_G, want, kw, fpv[k]);
-        if (want) gid[k] = g;
-      }
-    }
-  }
+  hot_assign<G::HOT_G>(H, &sm->dict_n, &sm->dict_lock, G::HOT_G, live, gid, [&](int k, HotKey& kw) { G::key_words(rows[k], kw); });
   const int hot_n = __shfl_sync(0xFFFFFFFFu, (int)lds_acquire_u32(&sm->dict_n), 0);      // every gid of this warp is below it
   bool anyhot = false;
 #pragma unroll
@@ -389,7 +275,7 @@ __device__ __forceinline__ void jit_agg_dict_tile(const KernelArgs& K, const typ
         if (rows[k].live && gid[k] >= 0) av[k] = G::template acc<J>(rows[k]);
       }
       hot_fold<G::RPT>(H, G::HOT_G, G::N_ACCS, hot_n, G::KEY_WORDS, G::acc_op(J), G::acc_word(J), J, G::acc_seen(J) != 0, av, gid,
-                       [&](int g) { return jit_hot_entry<G>(K, H, g); });
+                       jit_entry_of<G>(K, H));
     });
   }
   bool anycold = false;
@@ -427,65 +313,16 @@ __device__ __forceinline__ void jit_store_tile(const KernelArgs& K, const typena
 template <class G>
 __device__ __forceinline__ void jit_compact_tile(const KernelArgs& K, const typename G::Row (&rows)[G::RPT], JitSmem* sm, int64_t tile) {
   const PipelineParams& P = K.P[0];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  bool keep[G::RPT]; uint32_t before[G::RPT];
+  bool keep[G::RPT];
 #pragma unroll
-  for (int k = 0; k < G::RPT; ++k) {
-    keep[k] = rows[k].live;
-    const uint32_t b = __ballot_sync(0xFFFFFFFFu, keep[k]);
-    before[k] = __popc(b & ((1u << lane) - 1));
-    if (lane == 0) sm->warp_sums[k * JIT_NWARPS + warp] = __popc(b);
-  }
-  __syncthreads();
-  if (warp == 0) {
-    constexpr int n = G::RPT * JIT_NWARPS;
-    uint32_t v = lane < n ? sm->warp_sums[lane] : 0, incl = v;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, d); if (lane >= d) incl += t; }
-    if (lane < n) sm->warp_sums[lane] = incl - v;
-    const uint32_t total = __shfl_sync(0xFFFFFFFFu, incl, 31);
-    unsigned long long excl = 0;
-    if (P.tile_offsets) {
-      excl = P.tile_offsets[tile];
-    } else if (tile > 0) {
-      if (lane == 0) st_release_u64(P.tile_status + tile, (1ull << 62) | total);
-      int64_t hi = tile - 1;
-      uint32_t spins = 0;
-      for (;;) {
-        const int64_t t = hi - lane;
-        unsigned long long sw = t >= 0 ? ld_acquire_u64(P.tile_status + t) : (2ull << 62);
-        const unsigned flag = (unsigned)(sw >> 62);
-        const unsigned ready = __ballot_sync(0xFFFFFFFFu, flag != 0);
-        const unsigned prefix = __ballot_sync(0xFFFFFFFFu, flag == 2);
-        const int first_prefix = prefix ? __ffs(prefix) - 1 : 32;
-        const unsigned need = first_prefix >= 31 ? 0xFFFFFFFFu : ((2u << first_prefix) - 1);
-        if ((ready & need) != need) { if (++spins > (1u << 24)) __trap(); continue; }
-        unsigned long long vv = (lane <= first_prefix) ? (sw & ((1ull << 62) - 1)) : 0ull;
-#pragma unroll
-        for (int d = 16; d; d >>= 1) vv += __shfl_xor_sync(0xFFFFFFFFu, vv, d);
-        excl += vv;
-        if (first_prefix < 32) break;
-        hi -= 32;
-      }
-    }
-    if (lane == 0) {
-      sm->tile_base = excl;
-      if (!P.tile_offsets) {
-        st_release_u64(P.tile_status + tile, (2ull << 62) | (excl + total));
-        if ((tile + 1) * (int64_t)G::TILE >= P.n_rows) *P.out_count = excl + total;
-      }
-    }
-  }
-  __syncthreads();
-  const unsigned long long base = sm->tile_base;
-  uint32_t wbase[G::RPT];
-#pragma unroll
-  for (int k = 0; k < G::RPT; ++k) wbase[k] = sm->warp_sums[k * JIT_NWARPS + warp];
+  for (int k = 0; k < G::RPT; ++k) keep[k] = rows[k].live;
+  uint32_t at[G::RPT];
+  const unsigned long long base = compact_positions<G::RPT>(P, keep, tile, G::TILE, sm->warp_sums, &sm->tile_base, at);
   static_for<0, G::N_OUT>([&](auto Jc) { constexpr int J = decltype(Jc)::value;
 #pragma unroll
     for (int k = 0; k < G::RPT; ++k) {
       if (!keep[k]) continue;
-      const int64_t pos = (int64_t)(base + wbase[k] + before[k]);
+      const int64_t pos = (int64_t)(base + at[k]);
       if constexpr (G::out_width(J) != 0) G::template store<J>(rows[k], P.out[J].data, pos);
       else P.out[J].data[pos] = G::template out_bool<J>(rows[k]) ? 1 : 0;
       if constexpr (G::out_nullable(J) != 0) P.out[J].valid_bytes[pos] = G::template out_valid<J>(rows[k]) ? 1 : 0;
@@ -620,7 +457,7 @@ __device__ __forceinline__ void jit_main(const KernelArgs& K) {
     const HotDict H = hot_dict(scratch, G::HOT_G);
     if constexpr (G::AGG_TIER == 2) reg_flush(H, G::N_ACCS, R);
     hot_flush(H, &sm->dict_n, G::HOT_G, G::N_ACCS, G::KEY_WORDS, [](int j) { return G::acc_op(j); }, [](int j) { return G::acc_word(j); },
-              [&](int g) { return jit_hot_entry<G>(K, H, g); });
+              jit_entry_of<G>(K, H));
   }
 }
 

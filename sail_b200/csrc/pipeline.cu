@@ -740,77 +740,16 @@ __device__ __forceinline__ void load_tile_generic(const PipelineParams& P, uint8
 // ================================================================================================
 
 
-// state word: 0 = empty, else (tag30 << 2) | {1 = being written, 2 = ready}.  Carrying the tag in the
-// state lets a thread skip a slot that is being written for a different key without waiting on it.
-// `claimed` (optional) is set when this call inserted the key: exactly one caller per key sees it.
-__device__ __forceinline__ uint64_t* agg_find_or_insert(const AggParams& A, const KeyRegs& key, uint64_t h, uint32_t* err, bool* claimed = nullptr) {
-  const uint32_t tag = (uint32_t)(h >> 34) << 2;
-  uint64_t idx = h & A.capacity_mask;
-  uint64_t probes = 0;
-  uint32_t spins = 0;
-  while (probes <= A.capacity_mask) {
-    uint64_t* e = reinterpret_cast<uint64_t*>(A.table) + idx * A.entry_words;
-    uint32_t* st = A.state + idx;
-    uint32_t s = ld_acquire_u32(st);
-    if (s == ST_EMPTY) {
-      s = atomicCAS(st, ST_EMPTY, tag | ST_LOCKED);
-      if (s == ST_EMPTY) {
-        e[0] = h;
-        e[1] = 0;                                                   // seen
-        for (int w = 0; w < A.key_words; ++w) e[2 + w] = key.w[w];
-        for (int j = 0; j < A.n_accs; ++j)
-          for (int w = 0; w < acc_words_of(A.accs[j].op); ++w)
-            e[2 + A.key_words + A.accs[j].word + w] = acc_identity(A.accs[j].op, w);
-        st_release_u32(st, tag | ST_READY);                         // release: the entry words above are visible first
-        if (claimed) *claimed = true;
-        {
-          // occupied-slot list: one counter for the whole table, so the increment is aggregated over the lanes
-          // that insert in the same step (same-address atomics serialise in one L2 slice)
-          const unsigned m = __activemask();
-          const unsigned lane = threadIdx.x & 31;
-          const int lead = __ffs(m) - 1;
-          unsigned long long base = 0;
-          if ((int)lane == lead) base = atomicAdd(A.n_groups, (unsigned long long)__popc(m));
-          base = __shfl_sync(m, base, lead);
-          A.occ[base + __popc(m & ((1u << lane) - 1))] = (uint32_t)idx;
-        }
-        return e;
-      }
-    }
-    if ((s & ~3u) == tag) {
-      if ((s & 3u) == ST_LOCKED) {          // same tag, still being published: look again (bounded)
-        if (++spins > (1u << 24)) { atomicOr(err, ERR_TABLE_FULL); return nullptr; }
-        __nanosleep(32);
-        continue;
-      }
-      if (e[0] == h && key_words_equal(A.keys, A.n_keys, A.has_null_word, e + 2, key)) return e;
-    }
-    idx = (idx + 1) & A.capacity_mask;
-    ++probes;
-  }
-  atomicOr(err, ERR_TABLE_FULL);
-  return nullptr;
+// The interpreter's arguments to the group-table functions of agg_hot.cuh: identities from the accumulator descriptors, keys
+// compared by the key descriptors.
+__device__ __forceinline__ auto agg_init() {
+  return [](const AggParams& A, uint64_t* acc) {
+    for (int j = 0; j < A.n_accs; ++j)
+      for (int w = 0; w < acc_words_of(A.accs[j].op); ++w) acc[A.accs[j].word + w] = acc_identity(A.accs[j].op, w);
+  };
 }
-
-// Warp-cooperative front end: lanes of one warp that carry the same key hash elect a leader
-// (__match_any_sync); only leaders touch the table, followers receive the entry pointer by shuffle.
-// Removes same-warp contention on a slot that is being published.  All 32 lanes must call.
-// `claimed` (optional): this lane's key was inserted by this call -- by the lane itself, never for a follower.
-__device__ __forceinline__ uint64_t* agg_find_or_insert_warp(const AggParams& A, const KeyRegs& key, uint64_t h, bool need, uint32_t* err, bool* claimed = nullptr) {
-  const unsigned lane = threadIdx.x & 31;
-  const unsigned long long probe = need ? h : (0xFFFFFFFF00000000ull | lane);   // idle lanes match nobody useful
-  const unsigned peers = __match_any_sync(0xFFFFFFFFu, probe);
-  const int leader = __ffs(peers) - 1;
-  uint64_t* e = nullptr;
-  bool mine = false;
-  if (need && (int)lane == leader) e = agg_find_or_insert(A, key, h, err, &mine);
-  unsigned long long p = __shfl_sync(0xFFFFFFFFu, reinterpret_cast<unsigned long long>(e), leader);
-  uint64_t* got = reinterpret_cast<uint64_t*>(p);
-  // same hash but different key (64-bit collision inside one warp): fall back to an own lookup
-  if (need && (int)lane != leader && got && !key_words_equal(A.keys, A.n_keys, A.has_null_word, got + 2, key))
-    got = agg_find_or_insert(A, key, h, err, &mine);
-  if (claimed) *claimed = mine;
-  return need ? got : nullptr;
+__device__ __forceinline__ auto agg_eq() {
+  return [](const AggParams& A, const uint64_t* k, const KeyRegs& key) { return key_words_equal(A.keys, A.n_keys, A.has_null_word, k, key); };
 }
 
 // OP_DISTINCT_FIRST: the gate of a DISTINCT aggregate.  Every active row with a valid argument looks its (group key, argument)
@@ -828,7 +767,7 @@ __device__ __noinline__ void vm_distinct_first(const AggParams& D, const TileCtx
     KeyRegs key; bool hn; uint64_t h = 0;
     if (live) h = pack_key<MAX_KEYS>(D.keys, D.n_keys, 1, c, r, key, &hn);
     bool first = false;
-    agg_find_or_insert_warp(D, key, h, live, err, &first);
+    find_or_insert_warp<FROM_A, FROM_A>(D, key, h, live, err, agg_init(), agg_eq(), &first);
     pd[r] = first ? 1 : 0;
   }
 }
@@ -909,17 +848,13 @@ __device__ __forceinline__ void reg_pack(const AggParams& A, const TileCtx& c, i
 
 __device__ __forceinline__ HotDict hot_dict(const AggParams& A, uint8_t* arena) { return hot_dict(arena + A.hot_smem_off, A.hot_groups); }
 
-__device__ __noinline__ uint64_t* hot_entry(const PipelineParams& P, const AggParams& A, const HotDict H, int g) {
-  uint64_t* e = reinterpret_cast<uint64_t*>(H.entry[g]);
-  if (e) return e;
-  KeyRegs key;
-  for (int w = 0; w < MAX_KEY_WORDS; ++w) key.w[w] = (w < A.key_words && w < HOT_KEY_WORDS) ? H.keys[g * HOT_KEY_WORDS + w] : 0;
-  e = agg_find_or_insert(A, key, hash_packed_key(A, key), P.error_flag);
-  H.entry[g] = reinterpret_cast<uint64_t>(e);     // benign race: every writer stores the same pointer
-  return e;
+// entry_of(g): the table entry of dictionary group g (agg_hot.cuh: hot_entry)
+__device__ __forceinline__ auto agg_entry_of(const PipelineParams& P, const AggParams& A, const HotDict& H) {
+  return [&P, &A, H](int g) {
+    return hot_entry<FROM_A, FROM_A, KeyRegs>(H, g, A, P.error_flag,
+                              [](const AggParams& T, const KeyRegs& k) { return hash_packed_key(T, k); }, agg_init(), agg_eq());
+  };
 }
-
-
 
 // rows whose group is not in the CTA-local dictionary: global table, one warp-cooperative lookup per row slot
 
@@ -943,7 +878,7 @@ __device__ __noinline__ void agg_cold_rows(const PipelineParams& P, const AggPar
       const int r = threadIdx.x + k * NT;
       KeyRegs key; bool hn; uint64_t h = 0;
       if (cold) h = pack_key<MAX_KEYS>(A.keys, A.n_keys, A.has_null_word, c, r, key, &hn);
-      uint64_t* e = agg_find_or_insert_warp(A, key, h, cold, P.error_flag);
+      uint64_t* e = find_or_insert_warp<FROM_A, FROM_A>(A, key, h, cold, P.error_flag, agg_init(), agg_eq());
       if (cold && e) {
         for (int j = 0; j < A.n_accs; ++j) {
           const AccDesc& d = A.accs[j];
@@ -985,34 +920,8 @@ __device__ __forceinline__ void sink_agg(const PipelineParams& P, const AggParam
     gid[k] = -1;
   }
   if (A.hot_groups > 0) {
-    uint32_t fpv[RPT];
-    bool miss = false;
-    // other warps grow the dictionary meanwhile: lane 0's reading is broadcast so that the warp collectives below are executed
-    // by all lanes or by none
-    const int n0 = __shfl_sync(0xFFFFFFFFu, (int)lds_acquire_u32(&sm->dict_n), 0);
-#pragma unroll
-    for (int k = 0; k < RPT; ++k) {
-      fpv[k] = 0;
-      if (live[k]) {
-        HotKey kw;
-        reg_pack(A, c, threadIdx.x + k * NT, kw);
-        fpv[k] = hot_fp(kw);
-        gid[k] = hot_lookup<HOT_MAX_GROUPS>(H, n0, kw, fpv[k]);
-        miss |= gid[k] < 0;
-      }
-    }
-    if (n0 < A.hot_groups && __any_sync(0xFFFFFFFFu, miss)) {
-#pragma unroll
-      for (int k = 0; k < RPT; ++k) {
-        const bool want = live[k] && gid[k] < 0;
-        if (__any_sync(0xFFFFFFFFu, want)) {
-          HotKey kw;
-          reg_pack(A, c, threadIdx.x + k * NT, kw);
-          const int g = hot_dict_add<HOT_MAX_GROUPS>(H, &sm->dict_n, &sm->dict_lock, A.hot_groups, want, kw, fpv[k]);
-          if (want) gid[k] = g;
-        }
-      }
-    }
+    hot_assign<HOT_MAX_GROUPS>(H, &sm->dict_n, &sm->dict_lock, A.hot_groups, live, gid,
+                               [&](int k, HotKey& kw) { reg_pack(A, c, threadIdx.x + k * NT, kw); });
     const int hot_n = __shfl_sync(0xFFFFFFFFu, (int)lds_acquire_u32(&sm->dict_n), 0);      // every gid of this warp is below it
     bool anyhot = false;
 #pragma unroll
@@ -1026,8 +935,7 @@ __device__ __forceinline__ void sink_agg(const PipelineParams& P, const AggParam
           av[k].i = 0; av[k].f = 0.0; av[k].valid = false;
           if (gid[k] >= 0) av[k] = load_acc_value(d, c, threadIdx.x + k * NT);
         }
-        hot_fold<RPT>(H, A.hot_groups, A.n_accs, hot_n, A.key_words, d.op, d.word, j, d.track_seen != 0, av, gid,
-                      [&](int g) { return hot_entry(P, A, H, g); });
+        hot_fold<RPT>(H, A.hot_groups, A.n_accs, hot_n, A.key_words, d.op, d.word, j, d.track_seen != 0, av, gid, agg_entry_of(P, A, H));
       }
     }
   }
@@ -1046,35 +954,14 @@ __device__ __forceinline__ void sink_agg_reg(const PipelineParams& P, const AggP
   const uint8_t* pact = P.mask_slot == NO_SLOT ? nullptr : c.arena + P.mask_slot;
   const HotDict H = hot_dict(A, c.arena);
   int gid[RPT];
-  uint32_t fpv[RPT];
   bool live[RPT];
-  bool miss = false;
-  const int n0 = __shfl_sync(0xFFFFFFFFu, (int)lds_acquire_u32(&sm->dict_n), 0);      // warp-uniform (see sink_agg)
 #pragma unroll
   for (int k = 0; k < RPT; ++k) {
     const int r = threadIdx.x + k * NT;
     live[k] = r < c.nrows && (pact == nullptr || pact[r]);
-    gid[k] = -1; fpv[k] = 0;
-    if (live[k]) {
-      HotKey kw;
-      reg_pack(A, c, r, kw);
-      fpv[k] = hot_fp(kw);
-      gid[k] = hot_lookup<REG_GROUPS>(H, n0, kw, fpv[k]);
-      miss |= gid[k] < 0;
-    }
   }
-  if (n0 < REG_GROUPS && __any_sync(0xFFFFFFFFu, miss)) {
-#pragma unroll
-    for (int k = 0; k < RPT; ++k) {
-      const bool want = live[k] && gid[k] < 0;
-      if (__any_sync(0xFFFFFFFFu, want)) {
-        HotKey kw;
-        reg_pack(A, c, threadIdx.x + k * NT, kw);
-        const int g = hot_dict_add<REG_GROUPS>(H, &sm->dict_n, &sm->dict_lock, REG_GROUPS, want, kw, fpv[k]);
-        if (want) gid[k] = g;
-      }
-    }
-  }
+  hot_assign<REG_GROUPS>(H, &sm->dict_n, &sm->dict_lock, REG_GROUPS, live, gid,
+                         [&](int k, HotKey& kw) { reg_pack(A, c, threadIdx.x + k * NT, kw); });
   // accumulate: values first (RPT x n_accs loads), then predicated adds into the register partials
 #pragma unroll
   for (int k = 0; k < RPT; ++k) {
@@ -1095,30 +982,14 @@ __device__ __forceinline__ void sink_agg_reg(const PipelineParams& P, const AggP
             if (L.mode == 1) x = (i128)lds<int64_t>(p); else x = lds<i128>(p);
             if (fits55(x)) val[j] = (int64_t)x;
             else {                                            // rare: exact value straight to the table entry
-              uint64_t* e = hot_entry(P, A, H, gid[k]);
+              uint64_t* e = agg_entry_of(P, A, H)(gid[k]);
               // (an Int64 sum has one word and is defined mod 2^64: no carry into the next accumulator)
               if (e) acc_apply(A.accs[j].op, e + 2 + A.key_words + A.accs[j].word, i128_lo(x), i128_hi(x));
             }
           }
         }
       }
-      switch (gid[k]) {            // only this row's group is touched (divergent, but 4x fewer adds than predication)
-        case 0:
-#pragma unroll
-          for (int j = 0; j < REG_ACCS; ++j) R.v[0][j] += val[j];
-          break;
-        case 1:
-#pragma unroll
-          for (int j = 0; j < REG_ACCS; ++j) R.v[1][j] += val[j];
-          break;
-        case 2:
-#pragma unroll
-          for (int j = 0; j < REG_ACCS; ++j) R.v[2][j] += val[j];
-          break;
-        default:
-#pragma unroll
-          for (int j = 0; j < REG_ACCS; ++j) R.v[3][j] += val[j];
-      }
+      reg_add(R, gid[k], val);
     }
   }
   R.rows += RPT;
@@ -1174,73 +1045,24 @@ __device__ __forceinline__ void sink_store(const PipelineParams& P, const TileCt
   }
 }
 
-// look-back word: bits 63..62 = 0 invalid / 1 tile aggregate / 2 inclusive prefix
 template <int RPT>
-__device__ __forceinline__ void sink_compact(const PipelineParams& P, const TileCtx& c, Smem* sm, int tile) {
+__device__ __forceinline__ void sink_compact(const PipelineParams& P, const TileCtx& c, Smem* sm, int64_t tile) {
   const uint8_t* pact = P.mask_slot == NO_SLOT ? nullptr : c.arena + eff(c, P.mask_slot);
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  bool keep[RPT]; uint32_t before[RPT];
+  bool keep[RPT];
 #pragma unroll
   for (int k = 0; k < RPT; ++k) {
     const int r = threadIdx.x + k * NT;
     keep[k] = r < c.nrows && (pact == nullptr || pact[r]);
-    const uint32_t b = __ballot_sync(0xFFFFFFFFu, keep[k]);
-    before[k] = __popc(b & ((1u << lane) - 1));
-    if (lane == 0) sm->warp_sums[k * (NT / 32) + warp] = __popc(b);
   }
-  __syncthreads();
-  if (warp == 0) {
-    // exclusive scan of the RPT * 8 (<= 32) warp totals, in row order
-    const int n = RPT * (NT / 32);
-    uint32_t v = lane < n ? sm->warp_sums[lane] : 0, incl = v;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, d); if (lane >= d) incl += t; }
-    if (lane < n) sm->warp_sums[lane] = incl - v;
-    const uint32_t total = __shfl_sync(0xFFFFFFFFu, incl, 31);
-    // decoupled look-back, one warp wide: 32 predecessor tiles are inspected per step; the walk stops at the
-    // closest tile that already published an inclusive prefix (flag 2) and adds the aggregates (flag 1) in between
-    unsigned long long excl = 0;
-    if (P.tile_offsets) {
-      excl = P.tile_offsets[tile];             // two-pass filter: the mask pass already fixed every tile's position
-    } else if (tile > 0) {
-      if (lane == 0) st_release_u64(P.tile_status + tile, (1ull << 62) | total);
-      int hi = tile - 1;                       // newest tile not yet accounted for
-      uint32_t spins = 0;
-      for (;;) {
-        const int t = hi - lane;
-        unsigned long long sw = t >= 0 ? ld_acquire_u64(P.tile_status + t) : (2ull << 62);   // before tile 0: prefix 0
-        const unsigned flag = (unsigned)(sw >> 62);
-        const unsigned ready = __ballot_sync(0xFFFFFFFFu, flag != 0);
-        const unsigned prefix = __ballot_sync(0xFFFFFFFFu, flag == 2);
-        // usable window: lanes 0..first_prefix (inclusive) if all of them are ready
-        const int first_prefix = prefix ? __ffs(prefix) - 1 : 32;
-        const unsigned need = first_prefix >= 31 ? 0xFFFFFFFFu : ((2u << first_prefix) - 1);
-        if ((ready & need) != need) { if (++spins > (1u << 24)) __trap(); continue; }      // somebody in the window is not published yet
-        unsigned long long v = (lane <= first_prefix) ? (sw & ((1ull << 62) - 1)) : 0ull;
-#pragma unroll
-        for (int d = 16; d; d >>= 1) v += __shfl_xor_sync(0xFFFFFFFFu, v, d);
-        excl += v;
-        if (first_prefix < 32) break;          // reached a published prefix
-        hi -= 32;
-      }
-    }
-    if (lane == 0) {
-      sm->tile_base = excl;
-      if (!P.tile_offsets) {
-        st_release_u64(P.tile_status + tile, (2ull << 62) | (excl + total));
-        if ((int64_t)(tile + 1) * P.tile_rows >= P.n_rows) *P.out_count = excl + total;
-      }
-    }
-  }
-  __syncthreads();
-  const unsigned long long base = sm->tile_base;
+  uint32_t at[RPT];
+  const unsigned long long base = compact_positions<RPT>(P, keep, tile, P.tile_rows, sm->warp_sums, &sm->tile_base, at);
   for (int j = 0; j < P.n_out; ++j) {
     const OutputCol& o = P.out[j];
 #pragma unroll
     for (int k = 0; k < RPT; ++k) {
       if (!keep[k]) continue;
       const int r = threadIdx.x + k * NT;
-      const int64_t pos = (int64_t)(base + sm->warp_sums[k * (NT / 32) + warp] + before[k]);
+      const int64_t pos = (int64_t)(base + at[k]);
       if (o.width) store_value(o, c, r, pos);
       else o.data[pos] = c.arena[eff(c, o.slot) + r];                  // boolean column as bytes (packed later)
       if (o.valid_slot != NO_SLOT) o.valid_bytes[pos] = c.arena[eff(c, o.valid_slot) + r];
@@ -1606,7 +1428,7 @@ __global__ void __launch_bounds__(NT, MINB) pipeline_kernel(const __grid_constan
     } else {
       switch (P.sink) {
         case SINK_STORE: sink_store<RPT>(P, c); break;
-        case SINK_COMPACT: sink_compact<RPT>(P, c, sm, (int)cur_tile); break;
+        case SINK_COMPACT: sink_compact<RPT>(P, c, sm, cur_tile); break;
         case SINK_BUILD: sink_build<RPT>(P, aux->build, c, sm); break;
         case SINK_PARTITION: sink_partition<RPT>(P, aux->part, c); break;
         default: break;
@@ -1634,7 +1456,7 @@ __global__ void __launch_bounds__(NT, MINB) pipeline_kernel(const __grid_constan
     const HotDict H = hot_dict(A, arena);
     if (A.reg_path) reg_flush(H, A.n_accs, R);
     hot_flush(H, &sm->dict_n, A.hot_groups, A.n_accs, A.key_words, [&](int j) { return (int)A.accs[j].op; }, [&](int j) { return (int)A.accs[j].word; },
-              [&](int g) { return hot_entry(P0, A, H, g); });
+              agg_entry_of(P0, A, H));
   }
 }
 
@@ -1647,7 +1469,7 @@ __global__ void agg_rehash_kernel(AggParams A, const uint8_t* old_table, const u
     const uint64_t* src = reinterpret_cast<const uint64_t*>(old_table) + (uint64_t)old_occ[i] * A.entry_words;
     KeyRegs key;
     for (int w = 0; w < A.key_words; ++w) key.w[w] = src[2 + w];
-    uint64_t* e = agg_find_or_insert(A, key, hash_packed_key(A, key), err);
+    uint64_t* e = find_or_insert<FROM_A, FROM_A>(A, key, hash_packed_key(A, key), err, agg_init(), agg_eq());
     if (!e) continue;
     e[1] = src[1];
     for (int w = 0; w < A.acc_words; ++w) e[2 + A.key_words + w] = src[2 + A.key_words + w];
@@ -1660,7 +1482,7 @@ __global__ void agg_migrate_kernel(AggParams A, AggMigrateMap M, const uint8_t* 
     KeyRegs key;
     for (int w = 0; w < MAX_KEY_WORDS; ++w) key.w[w] = 0;
     for (int w = 0; w < M.old_key_words; ++w) key.w[w + M.key_shift] = src[2 + w];
-    uint64_t* e = agg_find_or_insert(A, key, hash_packed_key(A, key), err);
+    uint64_t* e = find_or_insert<FROM_A, FROM_A>(A, key, hash_packed_key(A, key), err, agg_init(), agg_eq());
     if (!e) continue;
     uint64_t seen = 0;
     for (int j = 0; j < A.n_accs; ++j) {
